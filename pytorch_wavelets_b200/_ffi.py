@@ -26,7 +26,7 @@ SYMBOLS = [
     'b200w_dtcwt_inv_j2plus', 'b200w_scat_j1', 'b200w_dwt_forward',
 ]
 KERNEL_ENTRIES = SYMBOLS[5:13]
-# float64: the generic tile kernels and the 1-D row kernels compiled for double (csrc/k_f64.cu)
+# float64: the generic tile kernels and the 1-D row kernels instantiated for double (csrc/b200wave.cu, csrc/dwt1d.cu)
 F64_ENTRIES = ['b200w_dwt_afb2d', 'b200w_dwt_sfb2d', 'b200w_dwt_afb1d', 'b200w_dwt_sfb1d', 'b200w_dtcwt_fwd_j1',
                'b200w_dtcwt_fwd_j2plus', 'b200w_dtcwt_inv_j1', 'b200w_dtcwt_inv_j2plus', 'b200w_scat_j1']
 SYMBOLS = SYMBOLS + [s + '_generic' for s in KERNEL_ENTRIES] + [s + '_f64' for s in F64_ENTRIES] + [

@@ -2,26 +2,40 @@
 //
 // Build (see pytorch_wavelets_b200/_build.py): every .cu of this directory is compiled with
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -Xcompiler -fPIC -c
-// in parallel and linked into libb200wave.so.  This unit holds the C ABI and the generic tile kernels; the
-// streaming kernels live in k_*.cu behind fast_api.h.
+// in parallel and linked into libb200wave.so.  This unit holds the C ABI and the generic tile kernels in float and
+// double; the float32 streaming kernels live in k_*.cu behind fast_api.h.  Double precision (the `_f64` entry points,
+// for torch.float64 callers, as the reference computes in the default dtype) always runs the generic tile kernels:
+// same source, index logic and accumulation order as float, IEEE double arithmetic.
 #include <cuda_runtime.h>
 #include <stdio.h>
 
+#include <type_traits>
+
 #include "launch_params.h"
+#include "launch.cuh"
 #include "fast_api.h"
 
 namespace b200w {
 constexpr int NT = 256;
 // ---- __global__ wrappers of the generic tile bodies ---------------------------------------------
-extern __shared__ __align__(16) float g_smem[];
+extern __shared__ __align__(16) unsigned char g_smem[];   // one byte array, cast to T* by every instantiation
 
-__global__ void __launch_bounds__(NT) k_afb2d_tile(const __grid_constant__ AfbParams p) { afb2d_tile<NT>(p, blockIdx.x, g_smem); }
-__global__ void __launch_bounds__(NT) k_sfb2d_tile(const __grid_constant__ SfbParams p) { sfb2d_tile<NT>(p, blockIdx.x, g_smem); }
-__global__ void __launch_bounds__(NT) k_fwd_j1_tile(const __grid_constant__ DtParams p) { fwd_j1_tile<NT, false>(p, blockIdx.x, g_smem); }
-__global__ void __launch_bounds__(NT) k_scat_j1_tile(const __grid_constant__ DtParams p) { fwd_j1_tile<NT, true>(p, blockIdx.x, g_smem); }
-__global__ void __launch_bounds__(NT) k_fwd_j2plus_tile(const __grid_constant__ DtParams p) { fwd_j2plus_tile<NT>(p, blockIdx.x, g_smem); }
-__global__ void __launch_bounds__(NT) k_inv_j1_tile(const __grid_constant__ DtParams p) { inv_j1_tile<NT>(p, blockIdx.x, g_smem); }
-__global__ void __launch_bounds__(NT) k_inv_j2plus_tile(const __grid_constant__ DtParams p) { inv_j2plus_tile<NT>(p, blockIdx.x, g_smem); }
+template <class T> __global__ void __launch_bounds__(NT) k_afb2d_tile(const __grid_constant__ AfbParamsT<T> p) { afb2d_tile<NT>(p, blockIdx.x, reinterpret_cast<T*>(g_smem)); }
+template <class T> __global__ void __launch_bounds__(NT) k_sfb2d_tile(const __grid_constant__ SfbParamsT<T> p) { sfb2d_tile<NT>(p, blockIdx.x, reinterpret_cast<T*>(g_smem)); }
+template <class T> __global__ void __launch_bounds__(NT) k_fwd_j1_tile(const __grid_constant__ DtParamsT<T> p) { fwd_j1_tile<NT, false>(p, blockIdx.x, reinterpret_cast<T*>(g_smem)); }
+template <class T> __global__ void __launch_bounds__(NT) k_scat_j1_tile(const __grid_constant__ DtParamsT<T> p) { fwd_j1_tile<NT, true>(p, blockIdx.x, reinterpret_cast<T*>(g_smem)); }
+template <class T> __global__ void __launch_bounds__(NT) k_fwd_j2plus_tile(const __grid_constant__ DtParamsT<T> p) { fwd_j2plus_tile<NT>(p, blockIdx.x, reinterpret_cast<T*>(g_smem)); }
+template <class T> __global__ void __launch_bounds__(NT) k_inv_j1_tile(const __grid_constant__ DtParamsT<T> p) { inv_j1_tile<NT>(p, blockIdx.x, reinterpret_cast<T*>(g_smem)); }
+template <class T> __global__ void __launch_bounds__(NT) k_inv_j2plus_tile(const __grid_constant__ DtParamsT<T> p) { inv_j2plus_tile<NT>(p, blockIdx.x, reinterpret_cast<T*>(g_smem)); }
+
+// the one buffer behind b200w_last_cuda_error(), written by every launch of the library (launch.cuh)
+thread_local char g_last_cuda_error[256] = "";
+
+int check_cuda(cudaError_t e) {
+  if (e == cudaSuccess) return B200W_OK;
+  snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "%s: %s", cudaGetErrorName(e), cudaGetErrorString(e));
+  return B200W_ECUDA;
+}
 
 }  // namespace b200w
 
@@ -29,127 +43,92 @@ using namespace b200w;
 
 namespace {
 
-thread_local char g_last_cuda_error[256] = "";
-
-int check_launch() {
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "%s: %s", cudaGetErrorName(e), cudaGetErrorString(e));
-    return B200W_ECUDA;
-  }
-  return B200W_OK;
-}
-
-template <class K>
-int set_smem(K kernel, size_t bytes) {
-  if (bytes > 48 * 1024) {
-    if (bytes > 227 * 1024) return B200W_EFILTER;
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    if (e != cudaSuccess) {
-      snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "%s: %s", cudaGetErrorName(e), cudaGetErrorString(e));
-      return B200W_ECUDA;
+// One level of one transform: the float32 streaming kernel `try_fast` when it covers p (unless the caller asked for
+// the generic kernel), else the generic tile kernel.  Double precision always runs the tile kernel.
+template <class T, class P, class F, class K>
+int run_level(const P& p, bool generic, F try_fast, K tile, long long blocks, int smem_elems, void* stream) {
+  if constexpr (std::is_same_v<T, float>) {
+    if (!generic) {
+      const int rc = try_fast(p, (cudaStream_t)stream);
+      if (rc != fast::kNoFastPath) return rc ? rc : check_launch();
     }
   }
-  return 0;
+  return launch(tile, p, blocks, NT, (size_t)smem_elems * sizeof(T), stream);
 }
 
-template <class K, class P>
-int launch_tile(K kernel, const P& p, long long blocks, int smem_floats, void* stream) {
-  if (blocks == 0) return B200W_OK;
-  const size_t bytes = (size_t)smem_floats * sizeof(float);
-  int rc = set_smem(kernel, bytes);
-  if (rc) return rc;
-  kernel<<<(unsigned)blocks, NT, bytes, (cudaStream_t)stream>>>(p);
-  return check_launch();
+template <class T>
+int dwt_afb2d_impl(const T* x, long long x_plane_stride, int x_pitch, T* ll, long long ll_plane_stride, int ll_pitch,
+                   T* highs, int planes, int H, int W, const T* fw_lo, const T* fw_hi, int Lw, const T* fh_lo,
+                   const T* fh_hi, int Lh, int mode, void* stream, bool generic) {
+  AfbParamsT<T> p;
+  const int rc = build_afb(p, x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, planes, H, W, fw_lo,
+                           fw_hi, Lw, fh_lo, fh_hi, Lh, mode);
+  return rc ? rc : run_level<T>(p, generic, fast::try_launch_afb, k_afb2d_tile<T>,
+                                (long long)planes * p.tiles_x * p.tiles_y, afb_smem_floats(Lw, Lh), stream);
 }
 
-}  // namespace
-
-namespace {
-
-static int dwt_afb2d_impl(const float* x, long long x_plane_stride, int x_pitch, float* ll, long long ll_plane_stride,
-                    int ll_pitch, float* highs, int planes, int H, int W, const float* fw_lo, const float* fw_hi,
-                    int Lw, const float* fh_lo, const float* fh_hi, int Lh, int mode, void* stream, bool generic) {
-  AfbParams p;
-  int rc = build_afb(p, x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, planes, H, W, fw_lo,
-                     fw_hi, Lw, fh_lo, fh_hi, Lh, mode);
-  if (rc) return rc;
-  rc = generic ? fast::kNoFastPath : fast::try_launch_afb(p, (cudaStream_t)stream);
-  if (rc != fast::kNoFastPath) return rc ? rc : check_launch();
-  return launch_tile(k_afb2d_tile, p, (long long)planes * p.tiles_x * p.tiles_y, afb_smem_floats(Lw, Lh), stream);
+template <class T>
+int dwt_sfb2d_impl(const T* ll, long long ll_plane_stride, int ll_pitch, const T* highs, T* y, long long y_plane_stride,
+                   int y_pitch, int planes, int Hc, int Wc, int Ho, int Wo, const T* gh_lo, const T* gh_hi, int Lh,
+                   const T* gw_lo, const T* gw_hi, int Lw, int mode, void* stream, bool generic) {
+  SfbParamsT<T> p;
+  const int rc = build_sfb(p, ll, ll_plane_stride, ll_pitch, highs, y, y_plane_stride, y_pitch, planes, Hc, Wc, Ho, Wo,
+                           gh_lo, gh_hi, Lh, gw_lo, gw_hi, Lw, mode);
+  return rc ? rc : run_level<T>(p, generic, fast::try_launch_sfb, k_sfb2d_tile<T>,
+                                (long long)planes * p.tiles_x * p.tiles_y, sfb_smem_floats(Lh, Lw), stream);
 }
 
-static int dwt_sfb2d_impl(const float* ll, long long ll_plane_stride, int ll_pitch, const float* highs, float* y,
-                    long long y_plane_stride, int y_pitch, int planes, int Hc, int Wc, int Ho, int Wo,
-                    const float* gh_lo, const float* gh_hi, int Lh, const float* gw_lo, const float* gw_hi, int Lw,
-                    int mode, void* stream, bool generic) {
-  SfbParams p;
-  int rc = build_sfb(p, ll, ll_plane_stride, ll_pitch, highs, y, y_plane_stride, y_pitch, planes, Hc, Wc, Ho, Wo,
-                     gh_lo, gh_hi, Lh, gw_lo, gw_hi, Lw, mode);
-  if (rc) return rc;
-  rc = generic ? fast::kNoFastPath : fast::try_launch_sfb(p, (cudaStream_t)stream);
-  if (rc != fast::kNoFastPath) return rc ? rc : check_launch();
-  return launch_tile(k_sfb2d_tile, p, (long long)planes * p.tiles_x * p.tiles_y, sfb_smem_floats(Lh, Lw), stream);
+template <class T>
+int dtcwt_fwd_j1_impl(const T* x, long long x_plane_stride, int x_pitch, T* ll, long long ll_plane_stride, int ll_pitch,
+                      T* highs, const long long hs[6], int N, int C, int H, int W, const T* h0, int L0, const T* h1,
+                      int L1, int mode, void* stream, bool generic) {
+  DtParamsT<T> p;
+  const int rc = build_fwd_j1(p, x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, hs, N, C, H, W, h0,
+                              L0, h1, L1, mode);
+  return rc ? rc : run_level<T>(p, generic, fast::try_launch_fwd_j1, k_fwd_j1_tile<T>,
+                                (long long)N * C * p.tiles_x * p.tiles_y, fwdj1_smem_floats(L0, L1), stream);
 }
 
-static int dtcwt_fwd_j1_impl(const float* x, long long x_plane_stride, int x_pitch, float* ll, long long ll_plane_stride,
-                       int ll_pitch, float* highs, const long long hs[6], int N, int C, int H, int W,
-                       const float* h0, int L0, const float* h1, int L1, int mode, void* stream, bool generic) {
-  DtParams p;
-  int rc = build_fwd_j1(p, x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, hs, N, C, H, W, h0, L0,
-                        h1, L1, mode);
-  if (rc) return rc;
-  rc = generic ? fast::kNoFastPath : fast::try_launch_fwd_j1(p, (cudaStream_t)stream);
-  if (rc != fast::kNoFastPath) return rc ? rc : check_launch();
-  return launch_tile(k_fwd_j1_tile, p, (long long)N * C * p.tiles_x * p.tiles_y, fwdj1_smem_floats(L0, L1), stream);
+template <class T>
+int dtcwt_fwd_j2plus_impl(const T* x, long long x_plane_stride, int x_pitch, T* ll, long long ll_plane_stride,
+                          int ll_pitch, T* highs, const long long hs[6], int N, int C, int H, int W, const T* h0a,
+                          const T* h1a, const T* h0b, const T* h1b, int m, void* stream, bool generic) {
+  DtParamsT<T> p;
+  const int rc = build_fwd_j2plus(p, x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, hs, N, C, H, W,
+                                  h0a, h1a, h0b, h1b, m);
+  return rc ? rc : run_level<T>(p, generic, fast::try_launch_fwd_j2plus, k_fwd_j2plus_tile<T>,
+                                (long long)N * C * p.tiles_x * p.tiles_y, fwdj2_smem_floats(m), stream);
 }
 
-static int dtcwt_fwd_j2plus_impl(const float* x, long long x_plane_stride, int x_pitch, float* ll,
-                           long long ll_plane_stride, int ll_pitch, float* highs, const long long hs[6], int N,
-                           int C, int H, int W, const float* h0a, const float* h1a, const float* h0b,
-                           const float* h1b, int m, void* stream, bool generic) {
-  DtParams p;
-  int rc = build_fwd_j2plus(p, x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, hs, N, C, H, W,
-                            h0a, h1a, h0b, h1b, m);
-  if (rc) return rc;
-  rc = generic ? fast::kNoFastPath : fast::try_launch_fwd_j2plus(p, (cudaStream_t)stream);
-  if (rc != fast::kNoFastPath) return rc ? rc : check_launch();
-  return launch_tile(k_fwd_j2plus_tile, p, (long long)N * C * p.tiles_x * p.tiles_y, fwdj2_smem_floats(m), stream);
+template <class T>
+int dtcwt_inv_j1_impl(const T* ll, long long ll_plane_stride, int ll_pitch, const T* highs, const long long hs[6], T* y,
+                      long long y_plane_stride, int y_pitch, int N, int C, int H, int W, const T* g0, int L0,
+                      const T* g1, int L1, int mode, void* stream, bool generic) {
+  DtParamsT<T> p;
+  const int rc = build_inv_j1(p, ll, ll_plane_stride, ll_pitch, highs, hs, y, y_plane_stride, y_pitch, N, C, H, W, g0,
+                              L0, g1, L1, mode);
+  return rc ? rc : run_level<T>(p, generic, fast::try_launch_inv_j1, k_inv_j1_tile<T>,
+                                (long long)N * C * p.tiles_x * p.tiles_y, invj1_smem_floats(L0, L1), stream);
 }
 
-static int dtcwt_inv_j1_impl(const float* ll, long long ll_plane_stride, int ll_pitch, const float* highs,
-                       const long long hs[6], float* y, long long y_plane_stride, int y_pitch, int N, int C, int H,
-                       int W, const float* g0, int L0, const float* g1, int L1, int mode, void* stream, bool generic) {
-  DtParams p;
-  int rc = build_inv_j1(p, ll, ll_plane_stride, ll_pitch, highs, hs, y, y_plane_stride, y_pitch, N, C, H, W, g0, L0,
-                        g1, L1, mode);
-  if (rc) return rc;
-  rc = generic ? fast::kNoFastPath : fast::try_launch_inv_j1(p, (cudaStream_t)stream);
-  if (rc != fast::kNoFastPath) return rc ? rc : check_launch();
-  return launch_tile(k_inv_j1_tile, p, (long long)N * C * p.tiles_x * p.tiles_y, invj1_smem_floats(L0, L1), stream);
+template <class T>
+int dtcwt_inv_j2plus_impl(const T* ll, long long ll_plane_stride, int ll_pitch, const T* highs, const long long hs[6],
+                          T* y, long long y_plane_stride, int y_pitch, int N, int C, int H, int W, const T* g0a,
+                          const T* g1a, const T* g0b, const T* g1b, int m, void* stream, bool generic) {
+  DtParamsT<T> p;
+  const int rc = build_inv_j2plus(p, ll, ll_plane_stride, ll_pitch, highs, hs, y, y_plane_stride, y_pitch, N, C, H, W,
+                                  g0a, g1a, g0b, g1b, m);
+  return rc ? rc : run_level<T>(p, generic, fast::try_launch_inv_j2plus, k_inv_j2plus_tile<T>,
+                                (long long)N * C * p.tiles_x * p.tiles_y, invj2_smem_floats(m), stream);
 }
 
-static int dtcwt_inv_j2plus_impl(const float* ll, long long ll_plane_stride, int ll_pitch, const float* highs,
-                           const long long hs[6], float* y, long long y_plane_stride, int y_pitch, int N, int C,
-                           int H, int W, const float* g0a, const float* g1a, const float* g0b, const float* g1b,
-                           int m, void* stream, bool generic) {
-  DtParams p;
-  int rc = build_inv_j2plus(p, ll, ll_plane_stride, ll_pitch, highs, hs, y, y_plane_stride, y_pitch, N, C, H, W,
-                            g0a, g1a, g0b, g1b, m);
-  if (rc) return rc;
-  rc = generic ? fast::kNoFastPath : fast::try_launch_inv_j2plus(p, (cudaStream_t)stream);
-  if (rc != fast::kNoFastPath) return rc ? rc : check_launch();
-  return launch_tile(k_inv_j2plus_tile, p, (long long)N * C * p.tiles_x * p.tiles_y, invj2_smem_floats(m), stream);
-}
-
-static int scat_j1_impl(const float* x, float* z, float* dre_dr, float* dim_dr, int N, int C, int H, int W,
-                  const float* h0, int L0, const float* h1, int L1, int mode, float magbias, void* stream, bool generic) {
-  DtParams p;
-  int rc = build_scat_j1(p, x, z, dre_dr, dim_dr, N, C, H, W, h0, L0, h1, L1, mode, magbias);
-  if (rc) return rc;
-  rc = generic ? fast::kNoFastPath : fast::try_launch_scat_j1(p, (cudaStream_t)stream);
-  if (rc != fast::kNoFastPath) return rc ? rc : check_launch();
-  return launch_tile(k_scat_j1_tile, p, (long long)N * C * p.tiles_x * p.tiles_y, fwdj1_smem_floats(L0, L1), stream);
+template <class T>
+int scat_j1_impl(const T* x, T* z, T* dre_dr, T* dim_dr, int N, int C, int H, int W, const T* h0, int L0, const T* h1,
+                 int L1, int mode, T magbias, void* stream, bool generic) {
+  DtParamsT<T> p;
+  const int rc = build_scat_j1(p, x, z, dre_dr, dim_dr, N, C, H, W, h0, L0, h1, L1, mode, magbias);
+  return rc ? rc : run_level<T>(p, generic, fast::try_launch_scat_j1, k_scat_j1_tile<T>,
+                                (long long)N * C * p.tiles_x * p.tiles_y, fwdj1_smem_floats(L0, L1), stream);
 }
 
 }  // namespace
@@ -176,76 +155,124 @@ const char* b200w_last_cuda_error(void) { return g_last_cuda_error; }
 int b200w_dwt_coeff_len(int n, int flen, int mode) { return coeff_len(n, flen, mode); }
 int b200w_dwt_rec_len(int k, int flen, int mode) { return rec_len(k, flen, mode); }
 
+// ---- per-level entry points: float (streaming kernel when one applies), float generic, double ------------------
+
 int b200w_dwt_afb2d(const float* x, long long x_plane_stride, int x_pitch, float* ll, long long ll_plane_stride,
                     int ll_pitch, float* highs, int planes, int H, int W, const float* fw_lo, const float* fw_hi,
                     int Lw, const float* fh_lo, const float* fh_hi, int Lh, int mode, void* stream) {
-  return dwt_afb2d_impl(x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, planes, H, W, fw_lo, fw_hi, Lw, fh_lo, fh_hi, Lh, mode, stream, false);
+  return dwt_afb2d_impl<float>(x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, planes, H, W, fw_lo, fw_hi, Lw, fh_lo, fh_hi, Lh, mode, stream, false);
 }
 int b200w_dwt_afb2d_generic(const float* x, long long x_plane_stride, int x_pitch, float* ll, long long ll_plane_stride,
-                    int ll_pitch, float* highs, int planes, int H, int W, const float* fw_lo, const float* fw_hi,
-                    int Lw, const float* fh_lo, const float* fh_hi, int Lh, int mode, void* stream) {
-  return dwt_afb2d_impl(x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, planes, H, W, fw_lo, fw_hi, Lw, fh_lo, fh_hi, Lh, mode, stream, true);
+                            int ll_pitch, float* highs, int planes, int H, int W, const float* fw_lo, const float* fw_hi,
+                            int Lw, const float* fh_lo, const float* fh_hi, int Lh, int mode, void* stream) {
+  return dwt_afb2d_impl<float>(x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, planes, H, W, fw_lo, fw_hi, Lw, fh_lo, fh_hi, Lh, mode, stream, true);
+}
+int b200w_dwt_afb2d_f64(const double* x, long long x_plane_stride, int x_pitch, double* ll, long long ll_plane_stride,
+                        int ll_pitch, double* highs, int planes, int H, int W, const double* fw_lo, const double* fw_hi,
+                        int Lw, const double* fh_lo, const double* fh_hi, int Lh, int mode, void* stream) {
+  return dwt_afb2d_impl<double>(x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, planes, H, W, fw_lo, fw_hi, Lw, fh_lo, fh_hi, Lh, mode, stream, true);
 }
 
 int b200w_dwt_sfb2d(const float* ll, long long ll_plane_stride, int ll_pitch, const float* highs, float* y,
                     long long y_plane_stride, int y_pitch, int planes, int Hc, int Wc, int Ho, int Wo,
                     const float* gh_lo, const float* gh_hi, int Lh, const float* gw_lo, const float* gw_hi, int Lw,
                     int mode, void* stream) {
-  return dwt_sfb2d_impl(ll, ll_plane_stride, ll_pitch, highs, y, y_plane_stride, y_pitch, planes, Hc, Wc, Ho, Wo, gh_lo, gh_hi, Lh, gw_lo, gw_hi, Lw, mode, stream, false);
+  return dwt_sfb2d_impl<float>(ll, ll_plane_stride, ll_pitch, highs, y, y_plane_stride, y_pitch, planes, Hc, Wc, Ho, Wo, gh_lo, gh_hi, Lh, gw_lo, gw_hi, Lw, mode, stream, false);
 }
 int b200w_dwt_sfb2d_generic(const float* ll, long long ll_plane_stride, int ll_pitch, const float* highs, float* y,
-                    long long y_plane_stride, int y_pitch, int planes, int Hc, int Wc, int Ho, int Wo,
-                    const float* gh_lo, const float* gh_hi, int Lh, const float* gw_lo, const float* gw_hi, int Lw,
-                    int mode, void* stream) {
-  return dwt_sfb2d_impl(ll, ll_plane_stride, ll_pitch, highs, y, y_plane_stride, y_pitch, planes, Hc, Wc, Ho, Wo, gh_lo, gh_hi, Lh, gw_lo, gw_hi, Lw, mode, stream, true);
+                            long long y_plane_stride, int y_pitch, int planes, int Hc, int Wc, int Ho, int Wo,
+                            const float* gh_lo, const float* gh_hi, int Lh, const float* gw_lo, const float* gw_hi, int Lw,
+                            int mode, void* stream) {
+  return dwt_sfb2d_impl<float>(ll, ll_plane_stride, ll_pitch, highs, y, y_plane_stride, y_pitch, planes, Hc, Wc, Ho, Wo, gh_lo, gh_hi, Lh, gw_lo, gw_hi, Lw, mode, stream, true);
+}
+int b200w_dwt_sfb2d_f64(const double* ll, long long ll_plane_stride, int ll_pitch, const double* highs, double* y,
+                        long long y_plane_stride, int y_pitch, int planes, int Hc, int Wc, int Ho, int Wo,
+                        const double* gh_lo, const double* gh_hi, int Lh, const double* gw_lo, const double* gw_hi, int Lw,
+                        int mode, void* stream) {
+  return dwt_sfb2d_impl<double>(ll, ll_plane_stride, ll_pitch, highs, y, y_plane_stride, y_pitch, planes, Hc, Wc, Ho, Wo, gh_lo, gh_hi, Lh, gw_lo, gw_hi, Lw, mode, stream, true);
 }
 
 int b200w_dtcwt_fwd_j1(const float* x, long long x_plane_stride, int x_pitch, float* ll, long long ll_plane_stride,
                        int ll_pitch, float* highs, const long long hs[6], int N, int C, int H, int W,
                        const float* h0, int L0, const float* h1, int L1, int mode, void* stream) {
-  return dtcwt_fwd_j1_impl(x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, hs, N, C, H, W, h0, L0, h1, L1, mode, stream, false);
+  return dtcwt_fwd_j1_impl<float>(x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, hs, N, C, H, W, h0, L0, h1, L1, mode, stream, false);
 }
 int b200w_dtcwt_fwd_j1_generic(const float* x, long long x_plane_stride, int x_pitch, float* ll, long long ll_plane_stride,
-                       int ll_pitch, float* highs, const long long hs[6], int N, int C, int H, int W,
-                       const float* h0, int L0, const float* h1, int L1, int mode, void* stream) {
-  return dtcwt_fwd_j1_impl(x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, hs, N, C, H, W, h0, L0, h1, L1, mode, stream, true);
+                               int ll_pitch, float* highs, const long long hs[6], int N, int C, int H, int W,
+                               const float* h0, int L0, const float* h1, int L1, int mode, void* stream) {
+  return dtcwt_fwd_j1_impl<float>(x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, hs, N, C, H, W, h0, L0, h1, L1, mode, stream, true);
+}
+int b200w_dtcwt_fwd_j1_f64(const double* x, long long x_plane_stride, int x_pitch, double* ll, long long ll_plane_stride,
+                           int ll_pitch, double* highs, const long long hs[6], int N, int C, int H, int W,
+                           const double* h0, int L0, const double* h1, int L1, int mode, void* stream) {
+  return dtcwt_fwd_j1_impl<double>(x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, hs, N, C, H, W, h0, L0, h1, L1, mode, stream, true);
 }
 
 int b200w_dtcwt_fwd_j2plus(const float* x, long long x_plane_stride, int x_pitch, float* ll,
                            long long ll_plane_stride, int ll_pitch, float* highs, const long long hs[6], int N,
                            int C, int H, int W, const float* h0a, const float* h1a, const float* h0b,
                            const float* h1b, int m, void* stream) {
-  return dtcwt_fwd_j2plus_impl(x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, hs, N, C, H, W, h0a, h1a, h0b, h1b, m, stream, false);
+  return dtcwt_fwd_j2plus_impl<float>(x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, hs, N, C, H, W, h0a, h1a, h0b, h1b, m, stream, false);
 }
 int b200w_dtcwt_fwd_j2plus_generic(const float* x, long long x_plane_stride, int x_pitch, float* ll,
-                           long long ll_plane_stride, int ll_pitch, float* highs, const long long hs[6], int N,
-                           int C, int H, int W, const float* h0a, const float* h1a, const float* h0b,
-                           const float* h1b, int m, void* stream) {
-  return dtcwt_fwd_j2plus_impl(x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, hs, N, C, H, W, h0a, h1a, h0b, h1b, m, stream, true);
+                                   long long ll_plane_stride, int ll_pitch, float* highs, const long long hs[6], int N,
+                                   int C, int H, int W, const float* h0a, const float* h1a, const float* h0b,
+                                   const float* h1b, int m, void* stream) {
+  return dtcwt_fwd_j2plus_impl<float>(x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, hs, N, C, H, W, h0a, h1a, h0b, h1b, m, stream, true);
+}
+int b200w_dtcwt_fwd_j2plus_f64(const double* x, long long x_plane_stride, int x_pitch, double* ll,
+                               long long ll_plane_stride, int ll_pitch, double* highs, const long long hs[6], int N,
+                               int C, int H, int W, const double* h0a, const double* h1a, const double* h0b,
+                               const double* h1b, int m, void* stream) {
+  return dtcwt_fwd_j2plus_impl<double>(x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, hs, N, C, H, W, h0a, h1a, h0b, h1b, m, stream, true);
 }
 
 int b200w_dtcwt_inv_j1(const float* ll, long long ll_plane_stride, int ll_pitch, const float* highs,
                        const long long hs[6], float* y, long long y_plane_stride, int y_pitch, int N, int C, int H,
                        int W, const float* g0, int L0, const float* g1, int L1, int mode, void* stream) {
-  return dtcwt_inv_j1_impl(ll, ll_plane_stride, ll_pitch, highs, hs, y, y_plane_stride, y_pitch, N, C, H, W, g0, L0, g1, L1, mode, stream, false);
+  return dtcwt_inv_j1_impl<float>(ll, ll_plane_stride, ll_pitch, highs, hs, y, y_plane_stride, y_pitch, N, C, H, W, g0, L0, g1, L1, mode, stream, false);
 }
 int b200w_dtcwt_inv_j1_generic(const float* ll, long long ll_plane_stride, int ll_pitch, const float* highs,
-                       const long long hs[6], float* y, long long y_plane_stride, int y_pitch, int N, int C, int H,
-                       int W, const float* g0, int L0, const float* g1, int L1, int mode, void* stream) {
-  return dtcwt_inv_j1_impl(ll, ll_plane_stride, ll_pitch, highs, hs, y, y_plane_stride, y_pitch, N, C, H, W, g0, L0, g1, L1, mode, stream, true);
+                               const long long hs[6], float* y, long long y_plane_stride, int y_pitch, int N, int C, int H,
+                               int W, const float* g0, int L0, const float* g1, int L1, int mode, void* stream) {
+  return dtcwt_inv_j1_impl<float>(ll, ll_plane_stride, ll_pitch, highs, hs, y, y_plane_stride, y_pitch, N, C, H, W, g0, L0, g1, L1, mode, stream, true);
+}
+int b200w_dtcwt_inv_j1_f64(const double* ll, long long ll_plane_stride, int ll_pitch, const double* highs,
+                           const long long hs[6], double* y, long long y_plane_stride, int y_pitch, int N, int C, int H,
+                           int W, const double* g0, int L0, const double* g1, int L1, int mode, void* stream) {
+  return dtcwt_inv_j1_impl<double>(ll, ll_plane_stride, ll_pitch, highs, hs, y, y_plane_stride, y_pitch, N, C, H, W, g0, L0, g1, L1, mode, stream, true);
 }
 
 int b200w_dtcwt_inv_j2plus(const float* ll, long long ll_plane_stride, int ll_pitch, const float* highs,
                            const long long hs[6], float* y, long long y_plane_stride, int y_pitch, int N, int C,
                            int H, int W, const float* g0a, const float* g1a, const float* g0b, const float* g1b,
                            int m, void* stream) {
-  return dtcwt_inv_j2plus_impl(ll, ll_plane_stride, ll_pitch, highs, hs, y, y_plane_stride, y_pitch, N, C, H, W, g0a, g1a, g0b, g1b, m, stream, false);
+  return dtcwt_inv_j2plus_impl<float>(ll, ll_plane_stride, ll_pitch, highs, hs, y, y_plane_stride, y_pitch, N, C, H, W, g0a, g1a, g0b, g1b, m, stream, false);
 }
 int b200w_dtcwt_inv_j2plus_generic(const float* ll, long long ll_plane_stride, int ll_pitch, const float* highs,
-                           const long long hs[6], float* y, long long y_plane_stride, int y_pitch, int N, int C,
-                           int H, int W, const float* g0a, const float* g1a, const float* g0b, const float* g1b,
-                           int m, void* stream) {
-  return dtcwt_inv_j2plus_impl(ll, ll_plane_stride, ll_pitch, highs, hs, y, y_plane_stride, y_pitch, N, C, H, W, g0a, g1a, g0b, g1b, m, stream, true);
+                                   const long long hs[6], float* y, long long y_plane_stride, int y_pitch, int N, int C,
+                                   int H, int W, const float* g0a, const float* g1a, const float* g0b, const float* g1b,
+                                   int m, void* stream) {
+  return dtcwt_inv_j2plus_impl<float>(ll, ll_plane_stride, ll_pitch, highs, hs, y, y_plane_stride, y_pitch, N, C, H, W, g0a, g1a, g0b, g1b, m, stream, true);
+}
+int b200w_dtcwt_inv_j2plus_f64(const double* ll, long long ll_plane_stride, int ll_pitch, const double* highs,
+                               const long long hs[6], double* y, long long y_plane_stride, int y_pitch, int N, int C,
+                               int H, int W, const double* g0a, const double* g1a, const double* g0b, const double* g1b,
+                               int m, void* stream) {
+  return dtcwt_inv_j2plus_impl<double>(ll, ll_plane_stride, ll_pitch, highs, hs, y, y_plane_stride, y_pitch, N, C, H, W, g0a, g1a, g0b, g1b, m, stream, true);
+}
+
+int b200w_scat_j1(const float* x, float* z, float* dre_dr, float* dim_dr, int N, int C, int H, int W,
+                  const float* h0, int L0, const float* h1, int L1, int mode, float magbias, void* stream) {
+  return scat_j1_impl<float>(x, z, dre_dr, dim_dr, N, C, H, W, h0, L0, h1, L1, mode, magbias, stream, false);
+}
+int b200w_scat_j1_generic(const float* x, float* z, float* dre_dr, float* dim_dr, int N, int C, int H, int W,
+                          const float* h0, int L0, const float* h1, int L1, int mode, float magbias, void* stream) {
+  return scat_j1_impl<float>(x, z, dre_dr, dim_dr, N, C, H, W, h0, L0, h1, L1, mode, magbias, stream, true);
+}
+int b200w_scat_j1_f64(const double* x, double* z, double* dre_dr, double* dim_dr, int N, int C, int H, int W,
+                      const double* h0, int L0, const double* h1, int L1, int mode, double magbias, void* stream) {
+  return scat_j1_impl<double>(x, z, dre_dr, dim_dr, N, C, H, W, h0, L0, h1, L1, mode, magbias, stream, true);
 }
 
 /* ---- whole-transform entry point: all J analysis levels of DWTForward.forward (reference dwt/transform2d.py:68-74) */
@@ -356,7 +383,7 @@ static int dwt_forward_impl(const float* x, long long x_plane_stride, int x_pitc
       if (rc == 0) rc = check_launch();
     }
     if (rc == fast::kNoFastPath)
-      rc = dwt_afb2d_impl(src, sps, spitch, ll, (long long)ho * wp, wp, highs[j], planes, h, w, fw_lo, fw_hi, Lw, fh_lo,
+      rc = dwt_afb2d_impl<float>(src, sps, spitch, ll, (long long)ho * wp, wp, highs[j], planes, h, w, fw_lo, fw_hi, Lw, fh_lo,
                           fh_hi, Lh, mode, stream, generic);
     if (rc) return rc;
     src = ll; sps = (long long)ho * wp; spitch = wp; h = ho; w = wo;
@@ -376,15 +403,6 @@ int b200w_dwt_forward_generic(const float* x, long long x_plane_stride, int x_pi
                               long long workspace_bytes, void* stream) {
   return dwt_forward_impl(x, x_plane_stride, x_pitch, planes, H, W, J, yl, highs, fw_lo, fw_hi, Lw, fh_lo, fh_hi, Lh,
                           mode, workspace, workspace_bytes, stream, true);
-}
-
-int b200w_scat_j1(const float* x, float* z, float* dre_dr, float* dim_dr, int N, int C, int H, int W,
-                  const float* h0, int L0, const float* h1, int L1, int mode, float magbias, void* stream) {
-  return scat_j1_impl(x, z, dre_dr, dim_dr, N, C, H, W, h0, L0, h1, L1, mode, magbias, stream, false);
-}
-int b200w_scat_j1_generic(const float* x, float* z, float* dre_dr, float* dim_dr, int N, int C, int H, int W,
-                  const float* h0, int L0, const float* h1, int L1, int mode, float magbias, void* stream) {
-  return scat_j1_impl(x, z, dre_dr, dim_dr, N, C, H, W, h0, L0, h1, L1, mode, magbias, stream, true);
 }
 
 }  // extern "C"

@@ -10,6 +10,7 @@
 #include <cuda_runtime.h>
 
 #include "common.h"
+#include "launch.cuh"
 
 namespace b200w {
 namespace prims {
@@ -24,11 +25,6 @@ struct PrimParams {
   int L, sym, along_w, highpass;
   PTaps<T> ha, hb;
 };
-
-__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ float fma_rn(float a, float b, float c) { return fmaf(a, b, c); }
-__device__ __forceinline__ double fma_rn(double a, double b, double c) { return fma(a, b, c); }
 
 // y[n] = sum_j h[j] x[ext(n + j - m)], m = L / 2, n in [0, N + 2m - L + 1)
 template <class T>
@@ -116,13 +112,11 @@ static int set_ptaps(PTaps<T>& d, const T* src, int L) {
 }
 
 template <class T, class K>
-static int launch(K kernel, PrimParams<T>& p, int planes, void* stream) {
+static int launch_prim(K kernel, PrimParams<T>& p, int planes, void* stream) {
   p.total = (long long)planes * p.Ho * p.Wo;
-  if (p.total == 0) return B200W_OK;
   const long long blocks = (p.total + 255) / 256;
   if (blocks > 2147483647LL) return B200W_ESIZE;
-  kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(p);
-  return cudaGetLastError() == cudaSuccess ? B200W_OK : B200W_ECUDA;
+  return launch(kernel, p, blocks, 256, 0, stream);
 }
 
 template <class T>
@@ -137,7 +131,7 @@ static int filter_impl(const T* x, T* y, int planes, int H, int W, const T* h, i
   const int ext = 2 * (L / 2) - L + 1;     // 0 for odd lengths, 1 for even ones
   p.x = x; p.y = y; p.H = H; p.W = W; p.Ho = along_w ? H : H + ext; p.Wo = along_w ? W + ext : W;
   p.L = L; p.sym = symmetric ? 1 : 0; p.along_w = along_w ? 1 : 0; p.highpass = 0;
-  return launch<T>(k_filter<T>, p, planes, stream);
+  return launch_prim<T>(k_filter<T>, p, planes, stream);
 }
 
 template <class T>
@@ -151,7 +145,7 @@ static int dfilt_impl(const T* x, T* y, int planes, int H, int W, const T* ha, c
   if ((rc = set_ptaps(p.ha, ha, m)) || (rc = set_ptaps(p.hb, hb, m))) return rc;
   p.x = x; p.y = y; p.H = H; p.W = W; p.Ho = along_w ? H : H / 2; p.Wo = along_w ? W / 2 : W;
   p.L = m; p.sym = 1; p.along_w = along_w ? 1 : 0; p.highpass = highpass ? 1 : 0;
-  return launch<T>(k_dfilt<T>, p, planes, stream);
+  return launch_prim<T>(k_dfilt<T>, p, planes, stream);
 }
 
 template <class T>
@@ -165,7 +159,7 @@ static int ifilt_impl(const T* x, T* y, int planes, int H, int W, const T* ha, c
   if ((rc = set_ptaps(p.ha, ha, m)) || (rc = set_ptaps(p.hb, hb, m))) return rc;
   p.x = x; p.y = y; p.H = H; p.W = W; p.Ho = along_w ? H : 2 * H; p.Wo = along_w ? 2 * W : W;
   p.L = m; p.sym = 1; p.along_w = along_w ? 1 : 0; p.highpass = highpass ? 1 : 0;
-  return launch<T>(k_ifilt<T>, p, planes, stream);
+  return launch_prim<T>(k_ifilt<T>, p, planes, stream);
 }
 
 }  // namespace prims

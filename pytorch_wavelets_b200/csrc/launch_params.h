@@ -24,7 +24,8 @@ inline int rec_len(int k, int flen, int mode) {
   return mode == B200W_MODE_PERIODIZATION ? 2 * k : 2 * k - flen + 2;
 }
 
-inline int set_taps(Taps& dst, const float* src, int L) {
+template <class T>
+inline int set_taps(TapsT<T>& dst, const T* src, int L) {
   if (!src) return B200W_EARG;
   if (L < 1 || L > kMaxTaps) return B200W_EFILTER;
   memset(&dst, 0, sizeof(dst));
@@ -37,9 +38,10 @@ inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 // Total CTA count must fit a 1-D grid.
 inline bool grid_ok(long long blocks) { return blocks >= 0 && blocks <= 2147483647LL; }
 
-inline int build_afb(AfbParams& p, const float* x, long long xps, int xpitch, float* ll, long long llps,
-                     int llpitch, float* highs, int planes, int H, int W, const float* fw_lo,
-                     const float* fw_hi, int Lw, const float* fh_lo, const float* fh_hi, int Lh, int mode) {
+template <class T>
+inline int build_afb(AfbParamsT<T>& p, const T* x, long long xps, int xpitch, T* ll, long long llps,
+                     int llpitch, T* highs, int planes, int H, int W, const T* fw_lo,
+                     const T* fw_hi, int Lw, const T* fh_lo, const T* fh_hi, int Lh, int mode) {
   if (!dwt_mode_ok(mode)) return B200W_EMODE;
   if (!x || !ll || !highs) return B200W_EARG;
   if (planes < 0 || H < 1 || W < 1) return B200W_ESIZE;
@@ -63,9 +65,10 @@ inline int build_afb(AfbParams& p, const float* x, long long xps, int xpitch, fl
   return 0;
 }
 
-inline int build_sfb(SfbParams& p, const float* ll, long long llps, int llpitch, const float* highs, float* y,
-                     long long yps, int ypitch, int planes, int Hc, int Wc, int Ho, int Wo, const float* gh_lo,
-                     const float* gh_hi, int Lh, const float* gw_lo, const float* gw_hi, int Lw, int mode) {
+template <class T>
+inline int build_sfb(SfbParamsT<T>& p, const T* ll, long long llps, int llpitch, const T* highs, T* y,
+                     long long yps, int ypitch, int planes, int Hc, int Wc, int Ho, int Wo, const T* gh_lo,
+                     const T* gh_hi, int Lh, const T* gw_lo, const T* gw_hi, int Lw, int mode) {
   if (!dwt_mode_ok(mode)) return B200W_EMODE;
   if (!ll || !y) return B200W_EARG;
   if (planes < 0 || Hc < 1 || Wc < 1) return B200W_ESIZE;
@@ -88,11 +91,13 @@ inline int build_sfb(SfbParams& p, const float* ll, long long llps, int llpitch,
   return 0;
 }
 
-inline void dt_clear(DtParams& p) { memset(&p, 0, sizeof(p)); }
+template <class T>
+inline void dt_clear(DtParamsT<T>& p) { memset(&p, 0, sizeof(p)); }
 
-inline int build_fwd_j1(DtParams& p, const float* x, long long xps, int xpitch, float* ll, long long llps,
-                        int llpitch, float* highs, const long long hs[6], int N, int C, int H, int W,
-                        const float* h0, int L0, const float* h1, int L1, int mode) {
+template <class T>
+inline int build_fwd_j1(DtParamsT<T>& p, const T* x, long long xps, int xpitch, T* ll, long long llps,
+                        int llpitch, T* highs, const long long hs[6], int N, int C, int H, int W,
+                        const T* h0, int L0, const T* h1, int L1, int mode) {
   dt_clear(p);
   if (!x || !ll) return B200W_EARG;
   if (highs && !hs) return B200W_EARG;
@@ -113,8 +118,9 @@ inline int build_fwd_j1(DtParams& p, const float* x, long long xps, int xpitch, 
   return 0;
 }
 
-inline int build_scat_j1(DtParams& p, const float* x, float* z, float* dre, float* dim, int N, int C, int H,
-                         int W, const float* h0, int L0, const float* h1, int L1, int mode, float magbias) {
+template <class T>
+inline int build_scat_j1(DtParamsT<T>& p, const T* x, T* z, T* dre, T* dim, int N, int C, int H,
+                         int W, const T* h0, int L0, const T* h1, int L1, int mode, T magbias) {
   dt_clear(p);
   if (!x || !z) return B200W_EARG;
   if ((dre == nullptr) != (dim == nullptr)) return B200W_EARG;
@@ -127,16 +133,17 @@ inline int build_scat_j1(DtParams& p, const float* x, float* z, float* dre, floa
   p.N = N; p.C = C; p.H = H; p.W = W; p.L0 = L0; p.L1 = L1;
   p.sym = (mode == B200W_MODE_SYMMETRIC);
   p.magbias = magbias;
-  p.magbias2 = (float)((double)magbias * (double)magbias);
+  p.magbias2 = (T)((double)magbias * (double)magbias);
   p.tiles_x = cdiv(W, kJ1TW);
   p.tiles_y = cdiv(H, kJ1TH);
   if (!grid_ok((long long)N * C * p.tiles_x * p.tiles_y)) return B200W_ESIZE;
   return 0;
 }
 
-inline int build_fwd_j2plus(DtParams& p, const float* x, long long xps, int xpitch, float* ll, long long llps,
-                            int llpitch, float* highs, const long long hs[6], int N, int C, int H, int W,
-                            const float* h0a, const float* h1a, const float* h0b, const float* h1b, int m) {
+template <class T>
+inline int build_fwd_j2plus(DtParamsT<T>& p, const T* x, long long xps, int xpitch, T* ll, long long llps,
+                            int llpitch, T* highs, const long long hs[6], int N, int C, int H, int W,
+                            const T* h0a, const T* h1a, const T* h0b, const T* h1b, int m) {
   dt_clear(p);
   if (!x || !ll) return B200W_EARG;
   if (highs && !hs) return B200W_EARG;
@@ -162,9 +169,10 @@ inline int build_fwd_j2plus(DtParams& p, const float* x, long long xps, int xpit
   return 0;
 }
 
-inline int build_inv_j1(DtParams& p, const float* ll, long long llps, int llpitch, const float* highs,
-                        const long long hs[6], float* y, long long yps, int ypitch, int N, int C, int H, int W,
-                        const float* g0, int L0, const float* g1, int L1, int mode) {
+template <class T>
+inline int build_inv_j1(DtParamsT<T>& p, const T* ll, long long llps, int llpitch, const T* highs,
+                        const long long hs[6], T* y, long long yps, int ypitch, int N, int C, int H, int W,
+                        const T* g0, int L0, const T* g1, int L1, int mode) {
   dt_clear(p);
   if (!y || (!ll && !highs)) return B200W_EARG;
   if (highs && !hs) return B200W_EARG;
@@ -175,7 +183,7 @@ inline int build_inv_j1(DtParams& p, const float* ll, long long llps, int llpitc
   if ((ll && llpitch < W) || ypitch < W) return B200W_EARG;
   p.in = ll; p.inps = llps; p.inpitch = llpitch;
   p.out = y; p.outps = yps; p.outpitch = ypitch;
-  p.highs = const_cast<float*>(highs);
+  p.highs = const_cast<T*>(highs);
   if (highs) for (int i = 0; i < 6; ++i) p.hs[i] = hs[i];
   p.N = N; p.C = C; p.H = H; p.W = W; p.L0 = L0; p.L1 = L1;
   p.sym = (mode == B200W_MODE_SYMMETRIC);
@@ -185,9 +193,10 @@ inline int build_inv_j1(DtParams& p, const float* ll, long long llps, int llpitc
   return 0;
 }
 
-inline int build_inv_j2plus(DtParams& p, const float* ll, long long llps, int llpitch, const float* highs,
-                            const long long hs[6], float* y, long long yps, int ypitch, int N, int C, int H,
-                            int W, const float* g0a, const float* g1a, const float* g0b, const float* g1b,
+template <class T>
+inline int build_inv_j2plus(DtParamsT<T>& p, const T* ll, long long llps, int llpitch, const T* highs,
+                            const long long hs[6], T* y, long long yps, int ypitch, int N, int C, int H,
+                            int W, const T* g0a, const T* g1a, const T* g0b, const T* g1b,
                             int m) {
   dt_clear(p);
   if (!y || (!ll && !highs)) return B200W_EARG;
@@ -201,7 +210,7 @@ inline int build_inv_j2plus(DtParams& p, const float* ll, long long llps, int ll
   if ((ll && llpitch < W) || ypitch < 2 * W) return B200W_EARG;
   p.in = ll; p.inps = llps; p.inpitch = llpitch;
   p.out = y; p.outps = yps; p.outpitch = ypitch;
-  p.highs = const_cast<float*>(highs);
+  p.highs = const_cast<T*>(highs);
   if (highs) for (int i = 0; i < 6; ++i) p.hs[i] = hs[i];
   p.N = N; p.C = C; p.H = H; p.W = W; p.L0 = m; p.L1 = m; p.sym = 1;
   p.tiles_x = cdiv(2 * W, kI2TW);

@@ -71,8 +71,8 @@ def test_missing_library_fails_loudly(monkeypatch, tmp_path):
 
 
 def test_f64_and_primitive_entries_validate_without_gpu(lib):
-    """The float64 and standalone-primitive entry points share the validation of the float32 ones (csrc/k_f64.cu compiles
-    launch_params.h for double; csrc/k_prims.cu checks sizes before launching)."""
+    """The float64 and standalone-primitive entry points share the validation of the float32 ones (launch_params.h is a
+    template on the element type; csrc/k_prims.cu checks sizes before launching)."""
     d = (ctypes.c_double * 10)(*([0.25] * 10))
     dp = ctypes.cast(d, ctypes.c_void_p)
     buf = ctypes.c_void_p(16)  # never dereferenced: validation fails first

@@ -1,6 +1,6 @@
 """float64 on the GPU: the reference computes in torch's default dtype (dwt/lowlevel.py:972, dtcwt/lowlevel.py:67; its
 tests run both precisions, tests/test_dwt.py:143-160, tests/test_dtcwt.py:116-135).  Here double-precision modules take
-the generic kernels compiled for double (csrc/k_f64.cu); they are compared with the float64 oracle at 1e-12."""
+the generic kernels instantiated for double (csrc/b200wave.cu, csrc/dwt1d.cu); they are compared with the float64 oracle at 1e-12."""
 import numpy as np
 import pytest
 import torch
