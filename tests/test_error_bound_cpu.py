@@ -1,5 +1,5 @@
 """The per-plane fp32 error bound of tests/util.py, checked on the CPU at the shapes and scales of
-tests/test_gpu_dtcwt_stream_sweep.py:
+tests/test_gpu_dtcwt_stream_sweep.py and tests/test_gpu_dwt_stream_sweep.py:
   soundness  the oracle's fp32 form and the host emulation of the shipped generic kernels (tests/emu) pass it against
              the float64 oracle evaluated on the same fp32 operands;
   tightness  one element of the smallest-scale plane moved by 1e-6 of that plane's scale fails it;
@@ -10,6 +10,7 @@ import pytest
 
 from oracle import oracle as orc
 from pytorch_wavelets_b200.dtcwt._tables import TABLES
+from pytorch_wavelets_b200.wavelets import Wavelet
 from tests import util
 from tests.emu import emu_backend as emu
 
@@ -106,7 +107,24 @@ def case_scat(biort, mode, magbias, shape=(2, 6, 38, 132), seed=5):
     return run, {'avg': b['avg'], 'mag': b['mag']}, s, sc
 
 
+def case_dwt_sfb2d(L, mode, has_hi=True, shape=(2, 6, 19, 37), seed=6):
+    """One DWT synthesis level with the dbL/2 synthesis filters (the filter lengths of the DWT stream sweep)."""
+    rng = np.random.default_rng(seed + L)
+    ll, sc = util.scaled_uniform(shape, rng)
+    hi, _ = util.scaled_uniform(shape[:2] + (3,) + shape[2:], rng, scales=sc)
+    hi = hi if has_hi else None
+    w = Wavelet('db%d' % (L // 2))
+    g0, g1 = _f32(w.rec_lo).astype(np.float64), _f32(w.rec_hi).astype(np.float64)
+    s = smax(ll, hi)
+
+    def run(impl, dt):
+        return {'y': impl.dwt_sfb2d(ll.astype(dt), None if hi is None else hi.astype(dt), *[g.astype(dt) for g in
+                                                                                             (g0, g1, g0, g1)], mode)}
+    return run, {'y': util.bound_sfb2d(g0, g1, g0, g1, has_hi) + (0.0,)}, s, sc
+
+
 INV_INPUTS = [(True, True), (False, True), (True, False)]   # (low-pass present, band-pass present)
+DWT_MODES = ('zero', 'symmetric', 'reflect', 'periodic', 'periodization')
 FAMILIES = {
     'fwd_j1': [lambda b=b, m=m: case_fwd_j1(b, m) for b in ('near_sym_a', 'near_sym_b', 'antonini', 'legall')
                for m in ('symmetric', 'zero')],
@@ -117,6 +135,8 @@ FAMILIES = {
                    for p in INV_INPUTS],
     'scat_j1': [lambda b=b, m=m, mb=mb: case_scat(b, m, mb) for b in ('near_sym_a', 'near_sym_b', 'antonini')
                 for m in ('symmetric', 'zero') for mb in (1e-2, 0.0)],
+    'dwt_sfb2d': [lambda L=L, m=m, h=h: case_dwt_sfb2d(L, m, h) for L in range(2, 21, 2) for m in DWT_MODES
+                  for h in (True, False)],
 }
 
 _WORST = {}

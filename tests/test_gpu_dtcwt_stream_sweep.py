@@ -14,7 +14,6 @@ largest plane.  Per case:
 and, once per instantiation, (d) NaN-filled outputs inside canaried buffers through the C ABI, and (e, one test) the kernel
 each case launches, read from a torch.profiler CUDA trace, is the one the dispatch rules predict."""
 import contextlib
-import re
 import zlib
 
 import numpy as np
@@ -26,7 +25,7 @@ from pytorch_wavelets_b200 import _ffi
 from pytorch_wavelets_b200.dtcwt import transform_funcs as tf
 from pytorch_wavelets_b200.dtcwt._tables import TABLES
 from pytorch_wavelets_b200.scatternet.lowlevel import scat_j1
-from tests import util
+from tests import sweep_util, util
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
@@ -77,27 +76,6 @@ def hla_i2(mq):
     return (h + 3) // 4 * 4
 
 
-def pick_chunks(base_items, rows_out, min_rows, pro, conc):
-    """stream_common.cuh pick_chunks: the number of row chunks of each (plane, strip) march."""
-    max_chunks = (rows_out + min_rows - 1) // min_rows
-    best, best_nc, last_ch = 0.0, 1, -1
-    for nc in range(1, min(max_chunks, 64) + 1):
-        ch = -(-rows_out // nc)
-        ch = -(-ch // min_rows) * min_rows
-        if ch == last_ch:
-            continue
-        last_ch = ch
-        n = -(-rows_out // ch)
-        cost = base_items * (rows_out + n * pro) / max(conc, 1) + 0.5 * (ch + pro)
-        if nc == 1 or cost < best:
-            best, best_nc = cost, n
-    return best_nc
-
-
-# resident one-warp CTAs on an H100: 1 .. 32 per SM on 132 SMs, whatever the kernel's occupancy
-CONC_RANGE = range(132, 132 * 32 + 1, 132)
-
-
 def chunk_counts(case):
     """(min, max) chunk count over every possible occupancy, from the kernel's own strip / chunk parameters."""
     N, C, H, W = case['shape']
@@ -108,8 +86,7 @@ def chunk_counts(case):
         items, rows, unit, pro = ((W // 4) + 31) // 32, H // 4, 4, 3
     else:
         items, rows, unit, pro = (W + 63) // 64, H // 2, 8, 8
-    counts = [pick_chunks(N * C * items, rows, unit, pro, c) for c in CONC_RANGE]
-    return min(counts), max(counts)
+    return sweep_util.chunk_range(N * C * items, rows, unit, pro)
 
 
 # ---- case matrices ---------------------------------------------------------------------------------------------------
@@ -120,8 +97,7 @@ J1_WIDTHS = [40, 64, 68, 256, 292]          # < 1 strip, 1 strip, 1 strip + 4 co
 J2_WIDTHS = [96, 128, 132, 384, 424]
 INV_WIDTHS = [40, 64, 68, 192, 228]
 SWEEP_NC = (2, 3)
-MANY_CHUNKS = 'many chunks'     # 1 x 2 planes, H >= 200: every march splits into many row chunks at any occupancy
-ONE_CHUNK = 'one chunk'         # 2000 small planes: every march is one chunk
+MANY_CHUNKS, ONE_CHUNK = sweep_util.MANY_CHUNKS, sweep_util.ONE_CHUNK
 
 
 _DEFAULTS = dict(mode=SYM, layout=(2, -1), pad=0, has_ll=True, has_hi=True, ll_trim=False, aux=False, magbias=1e-2,
@@ -447,23 +423,7 @@ def test_case_matrix_covers_the_kernels_and_both_chunk_regimes():
 
 # ---- (d) unwritten outputs and stray writes, through the C ABI ---------------------------------------------------------
 
-PAD = 77
-CANARY = 7.5
-
-
-class Canaried(object):
-    def __init__(self, shape):
-        n = int(np.prod(shape))
-        self.buf = torch.full((n + 2 * PAD,), CANARY, device=DEV)
-        self.buf[PAD:PAD + n] = float('nan')
-        self.t = self.buf[PAD:PAD + n].view(shape)
-
-    def ptr(self):
-        return self.t.data_ptr()
-
-    def check(self, what):
-        assert bool((self.buf[:PAD] == CANARY).all()) and bool((self.buf[-PAD:] == CANARY).all()), what + ': canary'
-        assert not bool(torch.isnan(self.t).any()), what + ': unwritten outputs'
+Canaried = sweep_util.Canaried
 
 
 @pytest.mark.parametrize('c', [c for c in CASES if c['canary']], ids=[c['id'] for c in CASES if c['canary']])
@@ -517,37 +477,18 @@ def test_canaries_and_unwritten_outputs(c):
 
 # ---- (e) which kernel each case launched -------------------------------------------------------------------------------
 
-_KNAME = re.compile(r'(fwd_j1_stream|fwd_j2plus_stream|inv_j1_stream|inv_j2plus_stream)<([^>]*)>'
-                    r'|k_(fwd_j1|fwd_j2plus|inv_j1|inv_j2plus|scat_j1)_tile')
-
-
-def _short(name):
-    m = _KNAME.search(name)
-    if not m:
-        return None
-    if m.group(1):
-        return '%s<%s>' % (m.group(1), m.group(2).replace(' ', ''))
-    return m.group(3) + '_tile'
+_short = sweep_util.kernel_namer(['fwd_j1_stream', 'fwd_j2plus_stream', 'inv_j1_stream', 'inv_j2plus_stream'],
+                                 ['fwd_j1', 'fwd_j2plus', 'inv_j1', 'inv_j2plus', 'scat_j1'])
 
 
 def test_dispatch_launches_the_expected_kernel():
     """One auto-dispatch call per case under a torch.profiler CUDA trace: the engine kernel it launched is the streaming
     instantiation the dispatch rules predict, or the generic tile kernel for the fallback cases -- so a width that
     silently fell back cannot turn test_stream_sweep's comparison with the generic kernel into a self-comparison."""
-    from torch.profiler import ProfilerActivity, profile
     prepared = [Prepared(c) for c in CASES]
-    torch.cuda.synchronize()
-    try:
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            for P in prepared:
-                P.run()
-            torch.cuda.synchronize()
-        events = [e for e in prof.events() if _short(e.name) is not None]
-    except Exception as e:   # (no CUPTI on this machine)
-        pytest.skip('CUDA activity tracing is unavailable: %s' % e)
-    if not events:
-        pytest.skip('CUDA activity tracing recorded no kernels')
-    seen = [_short(e.name) for e in sorted(events, key=lambda e: e.time_range.start)]
+    seen = sweep_util.traced_kernels(lambda: [P.run() for P in prepared], _short)
+    if seen is None:
+        pytest.skip('CUDA activity tracing is unavailable or recorded no kernels')
     want = [expected_kernel(c) for c in CASES]
     assert len(seen) == len(want), (len(seen), len(want))
     wrong = [(c['id'], w, s) for c, w, s in zip(CASES, want, seen) if w != s]

@@ -66,7 +66,7 @@ def l1(f):
 
 
 def l1_phase(f):
-    """Largest l1 norm of one interpolation phase (even or odd taps) of a q-shift synthesis filter."""
+    """Largest l1 norm of one interpolation phase (even or odd taps) of a synthesis filter."""
     f = np.asarray(f, dtype=np.float64).ravel()
     return max(l1(f[0::2]), l1(f[1::2]))
 
@@ -104,6 +104,19 @@ def bound_scat(h0, h1, magbias):
     a difference, whose rounding scales with r <= |w| + b: its bound gets magbias as an additive scale."""
     hG, hK = bound_fwd_j1(h0, h1)['highs']
     return {'avg': (l1(h0) ** 2, 3.0, 0.0), 'mag': (hG * SQRT2, 2.5, float(magbias)), 'band': (hG, hK)}
+
+
+def bound_sfb2d(gh_lo, gh_hi, gw_lo, gw_hi, has_hi=True):
+    """(G, K) of one DWT synthesis level (sfb2d).  An output sample is one interpolation phase of each filter along H
+    and along W, summed over the bands present: G = (sum of the per-phase l1 norms along H) x (the same along W).
+    The generic kernel / oracle run H then W, the streaming kernels W then H, each with a final add per pass.
+    K: 2.5 for 2 taps (every tap is 1/sqrt2, so G * s is reached and the roundings are a larger share of it), 1.5 for
+    longer filters, 2.0 for the low-pass band alone."""
+    nh = l1_phase(gh_lo) + (l1_phase(gh_hi) if has_hi else 0.0)
+    nw = l1_phase(gw_lo) + (l1_phase(gw_hi) if has_hi else 0.0)
+    if not has_hi:
+        return nh * nw, 2.0
+    return nh * nw, (2.5 if max(np.size(gh_lo), np.size(gw_lo)) <= 2 else 1.5)
 
 
 def planes_err_ratio(y, y64, s, G, K, add=0.0):
