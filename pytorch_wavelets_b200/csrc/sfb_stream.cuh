@@ -4,7 +4,7 @@
 namespace b200w {
 namespace fast {
 
-// fast_inverse.cuh -- streaming DWT synthesis kernel (included inside namespace b200w::fast).
+// sfb_stream.cuh -- streaming DWT synthesis kernels (included inside namespace b200w::fast).
 //
 // One warp owns 64 coefficient columns (= 128 output columns) of one plane and marches down the
 // coefficient rows.  The four subband rows (ll, lh, hl, hh) of each coefficient row are staged in a
@@ -265,19 +265,6 @@ __global__ void __launch_bounds__(32) sfb2d_stream(const __grid_constant__ SfbPa
 // STG.E.128 of the same registers to the same address as the scalar stores, and a fence after the ring zeroing did not
 // change the result, so a race elsewhere in the kernel that only this schedule exposes has not been ruled out.
 // ------------------------------------------------------------------------------------------------------------------
-#ifndef B200W_SFB4_NS
-#define B200W_SFB4_NS 2   /* ring depth in stages: 2 -> 10 KB per warp, 17 warps/SM (3: 15 KB, 14 warps) */
-#endif
-#ifndef B200W_SFB4_MINB
-#define B200W_SFB4_MINB 1
-#endif
-// (an explicit minBlocks of 1 is not neutral: ptxas then spends registers freely -- fwd_j2plus 156 -> 176, fwd_j1 96 -> 124 --
-// so the plain form is used unless a cap is asked for)
-#if B200W_SFB4_MINB > 1
-#define B200W_SFB4_LB __launch_bounds__(32, B200W_SFB4_MINB)
-#else
-#define B200W_SFB4_LB __launch_bounds__(32)
-#endif
 template <int L>
 struct Sfb4Cfg {
   static constexpr int HALF = L / 2;
@@ -286,7 +273,7 @@ struct Sfb4Cfg {
   static constexpr int SWB = (CW + HALF - 1 + 3) / 4 * 4;         // staged floats per band row (16-byte multiple)
   static constexpr int KR = (HALF % 2 == 0) ? 2 : 1;               // coefficient rows per stage
   static constexpr int UNS = HALF / KR;                            // window period in stages
-  static constexpr int NS = B200W_SFB4_NS;
+  static constexpr int NS = 2;                                     // ring depth in stages
   static constexpr int STAGE = KR * 4 * SWB;
   static constexpr int SMEM_BYTES = NS * STAGE * 4;
   static constexpr int NW = 4 + HALF - 1;                          // window of a lane in a band row
@@ -373,7 +360,7 @@ __device__ __forceinline__ void sfb4_stage_dispatch(int vv, const SfbParams& p, 
 }
 
 template <int L>
-__global__ void B200W_SFB4_LB sfb2d_stream4(const __grid_constant__ SfbParams p, int n_strips, int n_chunks,
+__global__ void __launch_bounds__(32) sfb2d_stream4(const __grid_constant__ SfbParams p, int n_strips, int n_chunks,
                                                     int CH /* output row pairs per chunk */) {
   using C = Sfb4Cfg<L>;
   extern __shared__ __align__(16) float ring[];
@@ -463,10 +450,6 @@ __global__ void B200W_SFB4_LB sfb2d_stream4(const __grid_constant__ SfbParams p,
   cp_async_wait<0>();
 }
 
-#ifndef B200W_SFB_WIDE
-#define B200W_SFB_WIDE 1
-#endif
-
 template <int L>
 inline int launch_sfb_stream4(const SfbParams& p, cudaStream_t stream, int n_strips) {
   using C = Sfb4Cfg<L>;
@@ -502,7 +485,7 @@ inline int launch_sfb_stream_m(const SfbParams& p, cudaStream_t stream) {
 template <int L>
 inline int launch_sfb_stream(const SfbParams& p, cudaStream_t stream) {
   if (p.mode == B200W_MODE_PERIODIZATION) return launch_sfb_stream_m<L, true>(p, stream);
-  if constexpr (L <= 8 && B200W_SFB_WIDE != 0) {
+  if constexpr (L <= 8) {
     // 128-column strips for every plane with more than 64 column pairs, remainder strip included: routing a narrow
     // remainder to the 2-column kernel in a second launch costs more than it saves, and one 67-pair wide strip beats a
     // 64 + 3 pair of narrow ones
