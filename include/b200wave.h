@@ -142,6 +142,55 @@ int b200w_dwt_sfb1d(const float* lo, const float* hi, int rows, int K, float* y,
                     const float* g0, const float* g1, int L, int mode, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * 3-D DWT levels (an addition beyond the reference; DWT3DForward / DWT3DInverse).  One filter pair acts along all
+ * three axes.  Analysis = the 1-D analysis along W, then H, then D, each pass rounded to the element type; synthesis is
+ * the reverse (along D, then the 2-D synthesis: H, then W).  Per axis the sizes follow b200w_dwt_coeff_len /
+ * b200w_dwt_rec_len.  Band b = 4*aW + 2*aH + aD - 1 (aX = 1: high-pass along X), so bands 1, 3, 5 are the 2-D
+ * lh, hl, hh of K1 low-passed along D and bands 0, 2, 4, 6 are high-pass along D.
+ *   b200w_dwt_afb3d: x (volumes, D, H, W), volume stride x_vol_stride elements (>= D*H*W), last three dims dense
+ *                    -> yl (volumes, Do, Ho, Wo) and highs (volumes, 7, Do, Ho, Wo), both contiguous.
+ *                    f_lo, f_hi: stored (reversed) analysis taps, length L.
+ *   b200w_dwt_sfb3d: yl (volumes, Dc, Hc, Wc) with volume stride yl_vol_stride (last three dims dense) and highs
+ *                    (volumes, 7, Dc, Hc, Wc) contiguous, or NULL = zeros (then it is never read)
+ *                    -> y (volumes, Do, Ho, Wo) contiguous.  Do / Ho / Wo may be smaller than the natural
+ *                    b200w_dwt_rec_len sizes: the crop of the analysis backward pass.  g_lo, g_hi: synthesis taps.
+ * Each also computes the other's backward pass when given the same stored filters.
+ * A float32 level with L in {2, 4, 6, 8} is one fused kernel that reads its input once and writes every output once;
+ * its workspace query returns 0.  Any other level takes the two-step route: the 2-D level (K1 / K2) over all
+ * volumes*D planes plus a 1-D pass along D, with intermediates in `workspace` (caller-owned device memory of at least
+ * the query's bytes; same arguments to both calls).  The _generic entries always take the two-step route (the A/B
+ * reference of the parity tests); the _f64 entries take it in double.
+ */
+long long b200w_dwt_afb3d_workspace(const float* x, long long x_vol_stride, int volumes, int D, int H, int W, int L,
+                                    int mode);
+int b200w_dwt_afb3d(const float* x, long long x_vol_stride, float* yl, float* highs, int volumes, int D, int H, int W,
+                    const float* f_lo, const float* f_hi, int L, int mode, void* workspace, long long workspace_bytes,
+                    void* stream);
+long long b200w_dwt_sfb3d_workspace(int volumes, int Dc, int Hc, int Wc, int Do, int Ho, int Wo, int L, int mode);
+int b200w_dwt_sfb3d(const float* yl, long long yl_vol_stride, const float* highs, float* y, int volumes, int Dc,
+                    int Hc, int Wc, int Do, int Ho, int Wo, const float* g_lo, const float* g_hi, int L, int mode,
+                    void* workspace, long long workspace_bytes, void* stream);
+long long b200w_dwt_afb3d_workspace_generic(const float* x, long long x_vol_stride, int volumes, int D, int H, int W,
+                                            int L, int mode);
+int b200w_dwt_afb3d_generic(const float* x, long long x_vol_stride, float* yl, float* highs, int volumes, int D, int H,
+                            int W, const float* f_lo, const float* f_hi, int L, int mode, void* workspace,
+                            long long workspace_bytes, void* stream);
+long long b200w_dwt_sfb3d_workspace_generic(int volumes, int Dc, int Hc, int Wc, int Do, int Ho, int Wo, int L,
+                                            int mode);
+int b200w_dwt_sfb3d_generic(const float* yl, long long yl_vol_stride, const float* highs, float* y, int volumes,
+                            int Dc, int Hc, int Wc, int Do, int Ho, int Wo, const float* g_lo, const float* g_hi, int L,
+                            int mode, void* workspace, long long workspace_bytes, void* stream);
+long long b200w_dwt_afb3d_workspace_f64(const double* x, long long x_vol_stride, int volumes, int D, int H, int W,
+                                        int L, int mode);
+int b200w_dwt_afb3d_f64(const double* x, long long x_vol_stride, double* yl, double* highs, int volumes, int D, int H,
+                        int W, const double* f_lo, const double* f_hi, int L, int mode, void* workspace,
+                        long long workspace_bytes, void* stream);
+long long b200w_dwt_sfb3d_workspace_f64(int volumes, int Dc, int Hc, int Wc, int Do, int Ho, int Wo, int L, int mode);
+int b200w_dwt_sfb3d_f64(const double* yl, long long yl_vol_stride, const double* highs, double* y, int volumes, int Dc,
+                        int Hc, int Wc, int Do, int Ho, int Wo, const double* g_lo, const double* g_hi, int L,
+                        int mode, void* workspace, long long workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * DTCWT.  "highs" is the reference's 6-D complex band-pass tensor; because o_dim / ri_dim are
  * configurable (dtcwt/transform_funcs.py:10-58) it is described by six ELEMENT strides
  * hs[6] = {n, c, orientation, row, col, real/imag}.  Default layout (N,C,6,H/2,W/2,2) is the

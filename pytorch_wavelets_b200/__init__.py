@@ -1,8 +1,9 @@
 """pytorch_wavelets_b200 -- H100 (sm_90a) engine for the 2-D wavelet filterbank hot path of
 fbcotter/pytorch_wavelets, behind the reference's nn.Module API.
 
-Same export list and aliases as the reference package (``pytorch_wavelets/__init__.py:1-36``) for the
-classes on the hot path and its direct callers (SURVEY.md section 8).
+The reference package's export list and aliases (``pytorch_wavelets/__init__.py:1-36``) for the classes on the
+hot path and its direct callers (SURVEY.md section 8), plus the 3-D DWT (``DWT3DForward`` / ``DWT3DInverse``,
+aliases ``DWT3D`` / ``IDWT3D``), which the reference does not have.
 Every transform runs in hand-written CUDA kernels through the C ABI of ``libb200wave.so``; there is no
 CPU or eager fallback.
 """
@@ -22,6 +23,10 @@ __all__ = [
     'DWT1DInverse',
     'DWT1D',
     'IDWT1D',
+    'DWT3DForward',
+    'DWT3DInverse',
+    'DWT3D',
+    'IDWT3D',
     'ScatLayer',
     'ScatLayerj2',
 ]
@@ -30,6 +35,7 @@ from pytorch_wavelets_b200._version import __version__
 from pytorch_wavelets_b200.dtcwt.transform2d import DTCWTForward, DTCWTInverse
 from pytorch_wavelets_b200.dwt.transform1d import DWT1DForward, DWT1DInverse
 from pytorch_wavelets_b200.dwt.transform2d import DWTForward, DWTInverse
+from pytorch_wavelets_b200.dwt.transform3d import DWT3DForward, DWT3DInverse
 from pytorch_wavelets_b200.scatternet import ScatLayer, ScatLayerj2
 
 # aliases, as in the reference
@@ -41,3 +47,5 @@ DWT2D = DWT
 IDWT2D = IDWT
 DWT1D = DWT1DForward
 IDWT1D = DWT1DInverse
+DWT3D = DWT3DForward
+IDWT3D = DWT3DInverse

@@ -33,7 +33,8 @@ SYMBOLS = SYMBOLS + [s + '_generic' for s in KERNEL_ENTRIES] + [s + '_f64' for s
     'b200w_dwt_forward_workspace', 'b200w_dwt_afb1d', 'b200w_dwt_sfb1d', 'b200w_comm_unique_id', 'b200w_comm_init', 'b200w_comm_destroy', 'b200w_allgather',
     'b200w_comm_last_error',
     'b200w_dtcwt_filter', 'b200w_dtcwt_dfilt', 'b200w_dtcwt_ifilt', 'b200w_dtcwt_filter_f64', 'b200w_dtcwt_dfilt_f64',
-    'b200w_dtcwt_ifilt_f64']
+    'b200w_dtcwt_ifilt_f64'] + [
+    'b200w_dwt_%s3d%s%s' % (d, w, v) for d in ('afb', 'sfb') for w in ('', '_workspace') for v in ('', '_generic', '_f64')]
 
 
 class B200WaveError(RuntimeError):
@@ -83,6 +84,15 @@ def lib():
                 getattr(L, 'b200w_dtcwt_filter' + sfx).argtypes = [c_vp, c_vp, c_int, c_int, c_int, pf, c_int, c_int, c_int, c_vp]
                 getattr(L, 'b200w_dtcwt_dfilt' + sfx).argtypes = [c_vp, c_vp, c_int, c_int, c_int, pf, pf, c_int, c_int, c_int, c_vp]
                 getattr(L, 'b200w_dtcwt_ifilt' + sfx).argtypes = [c_vp, c_vp, c_int, c_int, c_int, pf, pf, c_int, c_int, c_int, c_vp]
+        for v in ('', '_generic', '_f64'):   # 3-D levels (csrc/dwt3d.cu)
+            getattr(L, 'b200w_dwt_afb3d' + v).argtypes = [c_vp, c_ll, c_vp, c_vp, c_int, c_int, c_int, c_int,
+                                                          pf, pf, c_int, c_int, c_vp, c_ll, c_vp]
+            getattr(L, 'b200w_dwt_sfb3d' + v).argtypes = [c_vp, c_ll, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int,
+                                                          c_int, c_int, pf, pf, c_int, c_int, c_vp, c_ll, c_vp]
+            getattr(L, 'b200w_dwt_afb3d_workspace' + v).argtypes = [c_vp, c_ll] + [c_int] * 6
+            getattr(L, 'b200w_dwt_afb3d_workspace' + v).restype = c_ll
+            getattr(L, 'b200w_dwt_sfb3d_workspace' + v).argtypes = [c_int] * 9
+            getattr(L, 'b200w_dwt_sfb3d_workspace' + v).restype = c_ll
         for s in KERNEL_ENTRIES:
             getattr(L, s + '_generic').argtypes = getattr(L, s).argtypes
         for s in F64_ENTRIES:
@@ -226,6 +236,23 @@ def planes_view(t):
     else:
         ps = H * s[2]
     return t, int(ps), int(s[2])
+
+
+def volumes_view(t):
+    """(tensor, volume_stride) for a 5-D (N,C,D,H,W) tensor whose last three dims are dense and whose (N,C) dims
+    collapse to one volume index (a channel slice, a larger volume stride); copies to contiguous otherwise."""
+    N, C, D, H, W = t.shape
+
+    def vstride(s):
+        return s[1] if C > 1 else (s[0] if N > 1 else D * H * W)
+    s = t.stride()
+    ok = t.numel() > 0 and t[0, 0].is_contiguous() and vstride(s) >= D * H * W
+    if ok and N > 1 and C > 1:
+        ok = (s[0] == C * s[1])
+    if not ok:
+        t = t.contiguous()
+        s = t.stride()
+    return t, int(vstride(s))
 
 
 def stream_of(t):

@@ -202,6 +202,85 @@ def dwt_forward_levels(x, fw_lo, fw_hi, fh_lo, fh_hi, mode, J):
     return yl, yh
 
 
+def _taps_pair(f0, f1):
+    f0, f1 = _ffi.host_taps(f0), _ffi.host_taps(f1)
+    if f0.n != f1.n:
+        raise ValueError('low-pass and high-pass filters must have equal length')
+    return f0, f1
+
+
+def _workspace(like, nbytes, what):
+    if nbytes < 0:
+        _ffi.check(int(nbytes), what)
+    return like.new_empty(((nbytes + like.element_size() - 1) // like.element_size(),)) if nbytes > 0 else None
+
+
+def afb3d_level(x, h0, h1, mode):
+    """One 3-D analysis level on the GPU (``b200w_dwt_afb3d``): x (N,C,D,H,W) -> (yl (N,C,Do,Ho,Wo),
+    highs (N,C,7,Do,Ho,Wo)), both contiguous.  ``h0, h1``: stored (reversed) taps, applied along W, H and D.
+    Band b = 4*aW + 2*aH + aD - 1 (aX = 1: high-pass along X).  Honours ``_ffi.generic_kernels()``."""
+    if x.dim() != 5:
+        raise ValueError('expected a 5-D (N,C,D,H,W) input, got shape {}'.format(tuple(x.shape)))
+    dt = _ffi.require_cuda_real(x, 'x')
+    _check_bank_mode(mode)
+    L = _ffi.lib()
+    h0, h1 = _taps_pair(h0, h1)
+    N, C, D, H, W = x.shape
+    Do, Ho, Wo = [L.b200w_dwt_coeff_len(n, h0.n, mode) for n in (D, H, W)]
+    yl = x.new_empty((N, C, Do, Ho, Wo))
+    highs = x.new_empty((N, C, 7, Do, Ho, Wo))
+    if N * C > 0:
+        x, xvs = _ffi.volumes_view(x)
+        with torch.cuda.device(x.device):
+            wsb = _ffi.entry('b200w_dwt_afb3d_workspace', dt)(x.data_ptr(), xvs, N * C, D, H, W, h0.n, mode)
+            ws = _workspace(x, wsb, 'b200w_dwt_afb3d_workspace')
+            with _ffi.span('dwt_afb3d %dx%dx%d L%d' % (D, H, W, h0.n),
+                           x.element_size() * N * C * (D * H * W + 8 * Do * Ho * Wo)):
+                rc = _ffi.entry('b200w_dwt_afb3d', dt)(x.data_ptr(), xvs, yl.data_ptr(), highs.data_ptr(), N * C, D, H, W,
+                                                       h0.p(dt), h1.p(dt), h0.n, mode,
+                                                       None if ws is None else ws.data_ptr(), max(int(wsb), 0),
+                                                       _ffi.stream_of(x))
+        _ffi.check(rc, 'b200w_dwt_afb3d')
+    return yl, highs
+
+
+def sfb3d_level(yl, highs, g0, g1, mode, out_dhw=None):
+    """One 3-D synthesis level on the GPU (``b200w_dwt_sfb3d``): yl (N,C,Dc,Hc,Wc) and highs (N,C,7,Dc,Hc,Wc) or None
+    (zeros) -> y (N,C,Do,Ho,Wo).  ``out_dhw`` crops the output (the analysis backward pass)."""
+    if yl.dim() != 5:
+        raise ValueError('expected a 5-D (N,C,D,H,W) low-pass, got shape {}'.format(tuple(yl.shape)))
+    dt = _ffi.require_cuda_real(yl, 'low')
+    _check_bank_mode(mode)
+    L = _ffi.lib()
+    g0, g1 = _taps_pair(g0, g1)
+    N, C, Dc, Hc, Wc = yl.shape
+    if highs is not None:
+        _ffi.require_cuda_real(highs, 'highs', dt)
+        if tuple(highs.shape) != (N, C, 7, Dc, Hc, Wc):
+            raise ValueError('highs shape {} does not match low shape {}'.format(tuple(highs.shape), tuple(yl.shape)))
+        highs = highs.contiguous()
+    out = [L.b200w_dwt_rec_len(n, g0.n, mode) for n in (Dc, Hc, Wc)]
+    if out_dhw is not None:
+        out = [min(a, int(b)) for a, b in zip(out, out_dhw)]
+    if min(out) < 1:
+        raise ValueError('coefficient array {}x{}x{} too small for a {}-tap synthesis filter'.format(Dc, Hc, Wc, g0.n))
+    Do, Ho, Wo = out
+    y = yl.new_empty((N, C, Do, Ho, Wo))
+    if N * C > 0:
+        yl, ylvs = _ffi.volumes_view(yl)
+        with torch.cuda.device(yl.device):
+            wsb = _ffi.entry('b200w_dwt_sfb3d_workspace', dt)(N * C, Dc, Hc, Wc, Do, Ho, Wo, g0.n, mode)
+            ws = _workspace(yl, wsb, 'b200w_dwt_sfb3d_workspace')
+            with _ffi.span('dwt_sfb3d %dx%dx%d L%d' % (Dc, Hc, Wc, g0.n),
+                           yl.element_size() * N * C * ((1 if highs is None else 8) * Dc * Hc * Wc + Do * Ho * Wo)):
+                rc = _ffi.entry('b200w_dwt_sfb3d', dt)(yl.data_ptr(), ylvs, None if highs is None else highs.data_ptr(),
+                                                       y.data_ptr(), N * C, Dc, Hc, Wc, Do, Ho, Wo, g0.p(dt), g1.p(dt),
+                                                       g0.n, mode, None if ws is None else ws.data_ptr(),
+                                                       max(int(wsb), 0), _ffi.stream_of(yl))
+        _ffi.check(rc, 'b200w_dwt_sfb3d')
+    return y
+
+
 # ---- autograd Functions (the reference's drop-in boundary) ------------------------------------------------
 
 class AFB2D(Function):
@@ -290,3 +369,46 @@ class DWTPyramid(Function):
                 low = sfb2d_level(low.contiguous(), dyh[j], h0_col, h1_col, h0_row, h1_row, ctx.mode, out_hw=sh)
             dx = low
         return dx, None, None, None, None, None, None
+
+
+class AFB3D(Function):
+    """Single-level 3-D analysis: ``apply(x, h0, h1, mode) -> (yl, highs)`` with the stored (reversed) analysis taps
+    along all three axes.  The backward pass is the synthesis with the same stored taps, cropped to the input size
+    (as ``AFB2D.backward``)."""
+
+    @staticmethod
+    def forward(ctx, x, h0, h1, mode):
+        mode = int(mode)
+        int_to_mode(mode)
+        ctx.mode, ctx.shape = mode, tuple(x.shape[-3:])
+        ctx.taps = (_ffi.host_taps(h0), _ffi.host_taps(h1))
+        return afb3d_level(x, ctx.taps[0], ctx.taps[1], mode)
+
+    @staticmethod
+    def backward(ctx, dyl, dhighs):
+        dx = None
+        if ctx.needs_input_grad[0]:
+            dx = sfb3d_level(dyl.contiguous(), dhighs, ctx.taps[0], ctx.taps[1], ctx.mode, out_dhw=ctx.shape)
+        return dx, None, None, None
+
+
+class SFB3D(Function):
+    """Single-level 3-D synthesis: ``apply(yl, highs, g0, g1, mode) -> y``; ``highs`` may be None (zeros).  The
+    backward pass is the analysis with the synthesis taps (as ``SFB2D.backward``)."""
+
+    @staticmethod
+    def forward(ctx, yl, highs, g0, g1, mode):
+        mode = int(mode)
+        int_to_mode(mode)
+        ctx.mode, ctx.has_highs = mode, highs is not None
+        ctx.taps = (_ffi.host_taps(g0), _ffi.host_taps(g1))
+        return sfb3d_level(yl, highs, ctx.taps[0], ctx.taps[1], mode)
+
+    @staticmethod
+    def backward(ctx, dy):
+        dyl = dhighs = None
+        if ctx.needs_input_grad[0] or (ctx.has_highs and ctx.needs_input_grad[1]):
+            dyl, dhighs = afb3d_level(dy.contiguous(), ctx.taps[0], ctx.taps[1], ctx.mode)
+            if not ctx.has_highs:
+                dhighs = None
+        return dyl, dhighs, None, None, None
