@@ -191,6 +191,45 @@ int b200w_dwt_sfb3d_f64(const double* yl, long long yl_vol_stride, const double*
                         int mode, void* workspace, long long workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * 1-D DTCWT levels (an addition beyond the reference; DTCWT1DForward / DTCWT1DInverse).  Signals are `rows`
+ * independent rows; every output and the band-pass input are contiguous (rows, length) arrays.  Each call is one
+ * kernel that computes both filters of the level (both trees at levels >= 2).  Taps are stored (reversed) host arrays.
+ *   b200w_dtcwt1d_fwd_j1:     x (rows, n), row pitch x_pitch >= n -> lo, hi (rows, n); n even.
+ *                             lo = colfilter(x, h0), hi = colfilter(x, h1) along the row, mode symmetric or zero.
+ *                             h0 / h1 odd lengths L0 / L1.  hi may be NULL (skipped band-pass: nothing written).
+ *   b200w_dtcwt1d_fwd_j2plus: x (rows, n), n % 4 == 0 -> lo, hi (rows, n / 2);
+ *                             lo = coldfilt(x, h0b, h0a), hi = coldfilt(x, h1b, h1a, highpass); hi may be NULL.
+ *   b200w_dtcwt1d_inv_j1:     lo (rows, n) with row pitch lo_pitch >= n, hi (rows, n) -> y (rows, n); n even.
+ *                             y = colfilter(lo, g0) + colfilter(hi, g1).
+ *   b200w_dtcwt1d_inv_j2plus: lo (rows, n / 2) with row pitch lo_pitch, hi (rows, n / 2) -> y (rows, n), n % 4 == 0;
+ *                             y = colifilt(lo, g0b, g0a) + colifilt(hi, g1b, g1a, highpass).
+ *   The inverses take NULL for lo and / or hi (zeros: that branch is skipped) and round each branch before the sum.
+ * Errors: B200W_EARG for a NULL required pointer or a pitch below the row length, B200W_EMODE for a level-1 mode other
+ * than zero / symmetric, B200W_ESIZE for n odd (j1) or n % 4 != 0 (j2plus), B200W_EFILTER for an even or longer than
+ * B200W_MAX_TAPS level-1 filter or an odd / too long q-shift filter.  rows == 0 returns 0 without a launch.
+ */
+int b200w_dtcwt1d_fwd_j1(const float* x, long long x_pitch, int rows, int n, float* lo, float* hi,
+                         const float* h0, int L0, const float* h1, int L1, int mode, void* stream);
+int b200w_dtcwt1d_fwd_j2plus(const float* x, long long x_pitch, int rows, int n, float* lo, float* hi,
+                             const float* h0a, const float* h1a, const float* h0b, const float* h1b, int m,
+                             void* stream);
+int b200w_dtcwt1d_inv_j1(const float* lo, long long lo_pitch, const float* hi, int rows, int n, float* y,
+                         const float* g0, int L0, const float* g1, int L1, int mode, void* stream);
+int b200w_dtcwt1d_inv_j2plus(const float* lo, long long lo_pitch, const float* hi, int rows, int n, float* y,
+                             const float* g0a, const float* g1a, const float* g0b, const float* g1b, int m,
+                             void* stream);
+int b200w_dtcwt1d_fwd_j1_f64(const double* x, long long x_pitch, int rows, int n, double* lo, double* hi,
+                             const double* h0, int L0, const double* h1, int L1, int mode, void* stream);
+int b200w_dtcwt1d_fwd_j2plus_f64(const double* x, long long x_pitch, int rows, int n, double* lo, double* hi,
+                                 const double* h0a, const double* h1a, const double* h0b, const double* h1b, int m,
+                                 void* stream);
+int b200w_dtcwt1d_inv_j1_f64(const double* lo, long long lo_pitch, const double* hi, int rows, int n, double* y,
+                             const double* g0, int L0, const double* g1, int L1, int mode, void* stream);
+int b200w_dtcwt1d_inv_j2plus_f64(const double* lo, long long lo_pitch, const double* hi, int rows, int n, double* y,
+                                 const double* g0a, const double* g1a, const double* g0b, const double* g1b, int m,
+                                 void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * DTCWT.  "highs" is the reference's 6-D complex band-pass tensor; because o_dim / ri_dim are
  * configurable (dtcwt/transform_funcs.py:10-58) it is described by six ELEMENT strides
  * hs[6] = {n, c, orientation, row, col, real/imag}.  Default layout (N,C,6,H/2,W/2,2) is the

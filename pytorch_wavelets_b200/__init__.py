@@ -3,7 +3,8 @@ fbcotter/pytorch_wavelets, behind the reference's nn.Module API.
 
 The reference package's export list and aliases (``pytorch_wavelets/__init__.py:1-36``) for the classes on the
 hot path and its direct callers (SURVEY.md section 8), plus the 3-D DWT (``DWT3DForward`` / ``DWT3DInverse``,
-aliases ``DWT3D`` / ``IDWT3D``), which the reference does not have.
+aliases ``DWT3D`` / ``IDWT3D``) and the 1-D DTCWT (``DTCWT1DForward`` / ``DTCWT1DInverse``, aliases ``DTCWT1D`` /
+``IDTCWT1D``), which the reference does not have.
 Every transform runs in hand-written CUDA kernels through the C ABI of ``libb200wave.so``; there is no
 CPU or eager fallback.
 """
@@ -11,10 +12,14 @@ __all__ = [
     '__version__',
     'DTCWTForward',
     'DTCWTInverse',
+    'DTCWT1DForward',
+    'DTCWT1DInverse',
     'DWTForward',
     'DWTInverse',
     'DTCWT',
     'IDTCWT',
+    'DTCWT1D',
+    'IDTCWT1D',
     'DWT',
     'IDWT',
     'DWT2D',
@@ -32,6 +37,7 @@ __all__ = [
 ]
 
 from pytorch_wavelets_b200._version import __version__
+from pytorch_wavelets_b200.dtcwt.transform1d import DTCWT1DForward, DTCWT1DInverse
 from pytorch_wavelets_b200.dtcwt.transform2d import DTCWTForward, DTCWTInverse
 from pytorch_wavelets_b200.dwt.transform1d import DWT1DForward, DWT1DInverse
 from pytorch_wavelets_b200.dwt.transform2d import DWTForward, DWTInverse
@@ -41,6 +47,8 @@ from pytorch_wavelets_b200.scatternet import ScatLayer, ScatLayerj2
 # aliases, as in the reference
 DTCWT = DTCWTForward
 IDTCWT = DTCWTInverse
+DTCWT1D = DTCWT1DForward
+IDTCWT1D = DTCWT1DInverse
 DWT = DWTForward
 IDWT = DWTInverse
 DWT2D = DWT

@@ -34,7 +34,8 @@ SYMBOLS = SYMBOLS + [s + '_generic' for s in KERNEL_ENTRIES] + [s + '_f64' for s
     'b200w_comm_last_error',
     'b200w_dtcwt_filter', 'b200w_dtcwt_dfilt', 'b200w_dtcwt_ifilt', 'b200w_dtcwt_filter_f64', 'b200w_dtcwt_dfilt_f64',
     'b200w_dtcwt_ifilt_f64'] + [
-    'b200w_dwt_%s3d%s%s' % (d, w, v) for d in ('afb', 'sfb') for w in ('', '_workspace') for v in ('', '_generic', '_f64')]
+    'b200w_dwt_%s3d%s%s' % (d, w, v) for d in ('afb', 'sfb') for w in ('', '_workspace') for v in ('', '_generic', '_f64')] + [
+    'b200w_dtcwt1d_%s%s' % (k, v) for k in ('fwd_j1', 'fwd_j2plus', 'inv_j1', 'inv_j2plus') for v in ('', '_f64')]
 
 
 class B200WaveError(RuntimeError):
@@ -93,6 +94,15 @@ def lib():
             getattr(L, 'b200w_dwt_afb3d_workspace' + v).restype = c_ll
             getattr(L, 'b200w_dwt_sfb3d_workspace' + v).argtypes = [c_int] * 9
             getattr(L, 'b200w_dwt_sfb3d_workspace' + v).restype = c_ll
+        for v in ('', '_f64'):   # 1-D DTCWT levels (csrc/dtcwt1d.cu)
+            getattr(L, 'b200w_dtcwt1d_fwd_j1' + v).argtypes = [c_vp, c_ll, c_int, c_int, c_vp, c_vp, pf, c_int, pf, c_int,
+                                                               c_int, c_vp]
+            getattr(L, 'b200w_dtcwt1d_fwd_j2plus' + v).argtypes = [c_vp, c_ll, c_int, c_int, c_vp, c_vp, pf, pf, pf, pf,
+                                                                   c_int, c_vp]
+            getattr(L, 'b200w_dtcwt1d_inv_j1' + v).argtypes = [c_vp, c_ll, c_vp, c_int, c_int, c_vp, pf, c_int, pf, c_int,
+                                                               c_int, c_vp]
+            getattr(L, 'b200w_dtcwt1d_inv_j2plus' + v).argtypes = [c_vp, c_ll, c_vp, c_int, c_int, c_vp, pf, pf, pf, pf,
+                                                                   c_int, c_vp]
         for s in KERNEL_ENTRIES:
             getattr(L, s + '_generic').argtypes = getattr(L, s).argtypes
         for s in F64_ENTRIES:
