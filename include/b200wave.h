@@ -267,6 +267,28 @@ int b200w_dtcwt_fwd_j2plus(const float* x, long long x_plane_stride, int x_pitch
                            const float* h0b, const float* h1b, int m,
                            void* stream);
 
+/* K3+K4  levels 1 and 2 forward in one call: what b200w_dtcwt_fwd_j1 followed by b200w_dtcwt_fwd_j2plus on its
+ *     low-pass computes (bit for bit), without returning the level-1 low-pass.
+ *   x (N*C,H,W) pitched with H%4==0 and W%4==0 (else B200W_ESIZE); ll2 (N*C,H/2,W/2) pitched;
+ *   highs0 at (H/2,W/2) or NULL; highs1 at (H/4,W/4) or NULL; hs0 / hs1 their element strides as above.
+ *   h0o,h1o: stored level-1 filters (odd lengths L0, L1); h0a,h1a,h0b,h1b: stored q-shift filters (length m);
+ *   mode: level 1's extension as for b200w_dtcwt_fwd_j1.
+ *   When the fused kernel covers the call (highs0 given, 16-byte aligned rows, a compiled filter pair, a plane width
+ *   the kernel fits) the level-1 low-pass stays on chip and b200w_dtcwt_fwd_j12_workspace returns 0; otherwise it
+ *   returns the bytes of a float32 (N*C,H,W) low-pass and the two level kernels run through the caller's workspace
+ *   (B200W_EARG when it is missing or smaller).  The _generic form always runs the two generic tile levels and
+ *   always needs that workspace.  Validation as b200w_dtcwt_fwd_j1 / b200w_dtcwt_fwd_j2plus; N*C == 0 is a no-op.
+ */
+long long b200w_dtcwt_fwd_j12_workspace(const float* x, long long x_plane_stride, int x_pitch, const float* highs0,
+                                        int N, int C, int H, int W, int L0, int L1, int m);
+int b200w_dtcwt_fwd_j12(const float* x, long long x_plane_stride, int x_pitch,
+                        float* ll2, long long ll2_plane_stride, int ll2_pitch,
+                        float* highs0, const long long hs0[6], float* highs1, const long long hs1[6],
+                        int N, int C, int H, int W,
+                        const float* h0o, int L0, const float* h1o, int L1,
+                        const float* h0a, const float* h1a, const float* h0b, const float* h1b, int m,
+                        int mode, void* workspace, long long workspace_bytes, void* stream);
+
 /* K5  level-1 inverse.                     Replaces INV_J1.forward, transform_funcs.py:419-431
  *     (inv_j1 :152-184 = c2q (dtcwt/lowlevel.py:263-295), colfilter x4, rowfilter x2).
  *   ll (N*C,H,W) pitched or NULL (treated as zeros); highs at (H/2,W/2) or NULL (low-pass only
@@ -358,6 +380,13 @@ int b200w_dtcwt_fwd_j2plus_generic(const float* x, long long x_plane_stride, int
                                    float* highs, const long long hs[6], int N, int C, int H, int W,
                                    const float* h0a, const float* h1a, const float* h0b, const float* h1b,
                                    int m, void* stream);
+int b200w_dtcwt_fwd_j12_generic(const float* x, long long x_plane_stride, int x_pitch,
+                                float* ll2, long long ll2_plane_stride, int ll2_pitch,
+                                float* highs0, const long long hs0[6], float* highs1, const long long hs1[6],
+                                int N, int C, int H, int W,
+                                const float* h0o, int L0, const float* h1o, int L1,
+                                const float* h0a, const float* h1a, const float* h0b, const float* h1b, int m,
+                                int mode, void* workspace, long long workspace_bytes, void* stream);
 int b200w_dtcwt_inv_j1_generic(const float* ll, long long ll_plane_stride, int ll_pitch,
                                const float* highs, const long long hs[6],
                                float* y, long long y_plane_stride, int y_pitch, int N, int C, int H, int W,

@@ -35,7 +35,8 @@ SYMBOLS = SYMBOLS + [s + '_generic' for s in KERNEL_ENTRIES] + [s + '_f64' for s
     'b200w_dtcwt_filter', 'b200w_dtcwt_dfilt', 'b200w_dtcwt_ifilt', 'b200w_dtcwt_filter_f64', 'b200w_dtcwt_dfilt_f64',
     'b200w_dtcwt_ifilt_f64'] + [
     'b200w_dwt_%s3d%s%s' % (d, w, v) for d in ('afb', 'sfb') for w in ('', '_workspace') for v in ('', '_generic', '_f64')] + [
-    'b200w_dtcwt1d_%s%s' % (k, v) for k in ('fwd_j1', 'fwd_j2plus', 'inv_j1', 'inv_j2plus') for v in ('', '_f64')]
+    'b200w_dtcwt1d_%s%s' % (k, v) for k in ('fwd_j1', 'fwd_j2plus', 'inv_j1', 'inv_j2plus') for v in ('', '_f64')] + [
+    'b200w_dtcwt_fwd_j12', 'b200w_dtcwt_fwd_j12_generic', 'b200w_dtcwt_fwd_j12_workspace']
 
 
 class B200WaveError(RuntimeError):
@@ -103,6 +104,13 @@ def lib():
                                                                c_int, c_vp]
             getattr(L, 'b200w_dtcwt1d_inv_j2plus' + v).argtypes = [c_vp, c_ll, c_vp, c_int, c_int, c_vp, pf, pf, pf, pf,
                                                                    c_int, c_vp]
+        for v in ('', '_generic'):   # DTCWT forward levels 1 + 2 (csrc/dtcwt_fwd12.cuh)
+            getattr(L, 'b200w_dtcwt_fwd_j12' + v).argtypes = [c_vp, c_ll, c_int, c_vp, c_ll, c_int, c_vp, hs, c_vp, hs,
+                                                              c_int, c_int, c_int, c_int, pf, c_int, pf, c_int,
+                                                              pf, pf, pf, pf, c_int, c_int, c_vp, c_ll, c_vp]
+        L.b200w_dtcwt_fwd_j12_workspace.argtypes = [c_vp, c_ll, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
+                                                    c_int]
+        L.b200w_dtcwt_fwd_j12_workspace.restype = c_ll
         for s in KERNEL_ENTRIES:
             getattr(L, s + '_generic').argtypes = getattr(L, s).argtypes
         for s in F64_ENTRIES:

@@ -100,6 +100,36 @@ int dtcwt_fwd_j2plus_impl(const T* x, long long x_plane_stride, int x_pitch, T* 
                                 (long long)N * C * p.tiles_x * p.tiles_y, fwdj2_smem_floats(m), stream);
 }
 
+// DTCWT forward levels 1 and 2: the fused kernel when fwd12_route accepts the call (and the caller did not ask for the
+// generic kernels), else level 1 into the caller's LL1 workspace and level 2 from it.
+int dtcwt_fwd_j12_impl(const float* x, long long x_plane_stride, int x_pitch, float* ll2, long long ll2_plane_stride,
+                       int ll2_pitch, float* highs0, const long long hs0[6], float* highs1, const long long hs1[6], int N,
+                       int C, int H, int W, const float* h0o, int L0, const float* h1o, int L1, const float* h0a,
+                       const float* h1a, const float* h0b, const float* h1b, int m, int mode, void* workspace,
+                       long long workspace_bytes, void* stream, bool generic) {
+  DtParams p1, p2;
+  if (N >= 0 && C >= 1 && H >= 4 && W >= 4 && ((H & 3) || (W & 3))) return B200W_ESIZE;   // level 2's rule, up front
+  // (the LL1 pointers are not known yet: the builders only check them for null)
+  int rc = build_fwd_j1(p1, x, x_plane_stride, x_pitch, ll2, (long long)H * W, W, highs0, hs0, N, C, H, W, h0o, L0,
+                        h1o, L1, mode);
+  if (rc) return rc;
+  rc = build_fwd_j2plus(p2, x, (long long)H * W, W, ll2, ll2_plane_stride, ll2_pitch, highs1, hs1, N, C, H, W, h0a,
+                        h1a, h0b, h1b, m);
+  if (rc) return rc;
+  if ((long long)N * C == 0) return B200W_OK;
+  if (!generic) {
+    rc = fast::try_launch_fwd12(p1, p2, (cudaStream_t)stream);
+    if (rc != fast::kNoFastPath) return rc ? rc : check_launch();
+  }
+  if (!workspace || workspace_bytes < 4LL * N * C * H * W) return B200W_EARG;
+  float* ll1 = static_cast<float*>(workspace);
+  rc = dtcwt_fwd_j1_impl<float>(x, x_plane_stride, x_pitch, ll1, (long long)H * W, W, highs0, hs0, N, C, H, W, h0o, L0,
+                                h1o, L1, mode, stream, generic);
+  if (rc) return rc;
+  return dtcwt_fwd_j2plus_impl<float>(ll1, (long long)H * W, W, ll2, ll2_plane_stride, ll2_pitch, highs1, hs1, N, C, H,
+                                      W, h0a, h1a, h0b, h1b, m, stream, generic);
+}
+
 template <class T>
 int dtcwt_inv_j1_impl(const T* ll, long long ll_plane_stride, int ll_pitch, const T* highs, const long long hs[6], T* y,
                       long long y_plane_stride, int y_pitch, int N, int C, int H, int W, const T* g0, int L0,
@@ -225,6 +255,33 @@ int b200w_dtcwt_fwd_j2plus_f64(const double* x, long long x_plane_stride, int x_
                                int C, int H, int W, const double* h0a, const double* h1a, const double* h0b,
                                const double* h1b, int m, void* stream) {
   return dtcwt_fwd_j2plus_impl<double>(x, x_plane_stride, x_pitch, ll, ll_plane_stride, ll_pitch, highs, hs, N, C, H, W, h0a, h1a, h0b, h1b, m, stream, true);
+}
+
+long long b200w_dtcwt_fwd_j12_workspace(const float* x, long long x_plane_stride, int x_pitch, const float* highs0,
+                                        int N, int C, int H, int W, int L0, int L1, int m) {
+  if (N < 0 || C < 1 || H < 4 || W < 4 || (H & 3) || (W & 3)) return B200W_ESIZE;
+  Fwd12Plan pl;
+  if (fwd12_route(pl, x, x_plane_stride, x_pitch, H, W, L0, L1, m, highs0 != nullptr) == 0) return 0;
+  return 4LL * N * C * H * W;
+}
+int b200w_dtcwt_fwd_j12(const float* x, long long x_plane_stride, int x_pitch, float* ll2, long long ll2_plane_stride,
+                        int ll2_pitch, float* highs0, const long long hs0[6], float* highs1, const long long hs1[6],
+                        int N, int C, int H, int W, const float* h0o, int L0, const float* h1o, int L1,
+                        const float* h0a, const float* h1a, const float* h0b, const float* h1b, int m, int mode,
+                        void* workspace, long long workspace_bytes, void* stream) {
+  return dtcwt_fwd_j12_impl(x, x_plane_stride, x_pitch, ll2, ll2_plane_stride, ll2_pitch, highs0, hs0, highs1, hs1, N,
+                            C, H, W, h0o, L0, h1o, L1, h0a, h1a, h0b, h1b, m, mode, workspace, workspace_bytes, stream,
+                            false);
+}
+int b200w_dtcwt_fwd_j12_generic(const float* x, long long x_plane_stride, int x_pitch, float* ll2,
+                                long long ll2_plane_stride, int ll2_pitch, float* highs0, const long long hs0[6],
+                                float* highs1, const long long hs1[6], int N, int C, int H, int W, const float* h0o,
+                                int L0, const float* h1o, int L1, const float* h0a, const float* h1a, const float* h0b,
+                                const float* h1b, int m, int mode, void* workspace, long long workspace_bytes,
+                                void* stream) {
+  return dtcwt_fwd_j12_impl(x, x_plane_stride, x_pitch, ll2, ll2_plane_stride, ll2_pitch, highs0, hs0, highs1, hs1, N,
+                            C, H, W, h0o, L0, h1o, L1, h0a, h1a, h0b, h1b, m, mode, workspace, workspace_bytes, stream,
+                            true);
 }
 
 int b200w_dtcwt_inv_j1(const float* ll, long long ll_plane_stride, int ll_pitch, const float* highs,

@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 
 #include "common.h"
+#include "dtcwt_fwd12_plan.h"
 #include "pyramid_plan.h"
 
 namespace b200w {
@@ -20,6 +21,9 @@ int try_launch_scat_j1(const DtParams& p, cudaStream_t stream);
 int try_launch_fwd_j2plus(const DtParams& p, cudaStream_t stream);
 int try_launch_inv_j1(const DtParams& p, cudaStream_t stream);
 int try_launch_inv_j2plus(const DtParams& p, cudaStream_t stream);
+// DTCWT forward levels 1 and 2 in one kernel (k_dtcwt_fwd.cu): p1 = level 1 (its `out` unused), p2 = level 2 (its `in`
+// unused); kNoFastPath unless fwd12_route accepts the call
+int try_launch_fwd12(const DtParams& p1, const DtParams& p2, cudaStream_t stream);
 
 // fused multi-level DWT analysis (k_pyramid.cu): plan_dwt_pyramid fills everything but the output pointers and the
 // taps and returns kNoFastPath when the fused kernel does not apply (then run the levels one by one)

@@ -8,7 +8,8 @@ from numpy import ndarray
 from pytorch_wavelets_b200.dtcwt.coeffs import biort as _biort
 from pytorch_wavelets_b200.dtcwt.coeffs import qshift as _qshift
 from pytorch_wavelets_b200.dtcwt.lowlevel import prep_filt
-from pytorch_wavelets_b200.dtcwt.transform_funcs import FWD_J1, FWD_J2PLUS, INV_J1, INV_J2PLUS, get_dimensions6
+from pytorch_wavelets_b200.dtcwt.transform_funcs import (FWD_J1, FWD_J12, FWD_J2PLUS, INV_J1, INV_J2PLUS,
+                                                         get_dimensions6)
 from pytorch_wavelets_b200.dwt.lowlevel import mode_to_int
 
 
@@ -86,11 +87,21 @@ class DTCWTForward(nn.Module):
             x = torch.cat((x, x[:, :, -1:]), dim=2)
         if c % 2 != 0:
             x = torch.cat((x, x[:, :, :, -1:]), dim=3)
-        low, h = FWD_J1.apply(x, self.h0o, self.h1o, self.skip_hps[0], self.o_dim, self.ri_dim, mode)
-        highs[0] = h
-        if self.include_scale[0]:
-            scales[0] = low
-        for j in range(1, self.J):
+        j0 = 1
+        if (self.J >= 2 and x.dtype == torch.float32 and not self.include_scale[0] and not self.skip_hps[0]
+                and x.shape[2] % 4 == 0 and x.shape[3] % 4 == 0):
+            # levels 1 and 2 in one call: the level-1 low-pass is neither returned nor padded between the levels
+            low, highs[0], highs[1] = FWD_J12.apply(x, self.h0o, self.h1o, self.h0a, self.h1a, self.h0b, self.h1b,
+                                                    self.skip_hps[1], self.o_dim, self.ri_dim, mode)
+            if self.include_scale[1]:
+                scales[1] = low
+            j0 = 2
+        else:
+            low, h = FWD_J1.apply(x, self.h0o, self.h1o, self.skip_hps[0], self.o_dim, self.ri_dim, mode)
+            highs[0] = h
+            if self.include_scale[0]:
+                scales[0] = low
+        for j in range(j0, self.J):
             r, c = low.shape[2:]
             low = _replicate_pad(low, r % 4 != 0, c % 4 != 0)
             low, h = FWD_J2PLUS.apply(low, self.h0a, self.h1a, self.h0b, self.h1b, self.skip_hps[j],

@@ -138,6 +138,45 @@ def fwd_j2plus(x, h0a, h1a, h0b, h1b, skip_hps, o5, ri):
     return ll, highs
 
 
+def fwd_j12(x, h0o, h1o, h0a, h1a, h0b, h1b, skip_hps1, o5, ri, mode):
+    """Levels 1 and 2 in one call (float32, H % 4 == W % 4 == 0, level-1 band-pass kept): ll2, highs0, highs1 (None
+    when skipped), equal bit for bit to fwd_j1 followed by fwd_j2plus on its low-pass."""
+    if x.dtype != torch.float32:
+        raise NotImplementedError('the fused DTCWT levels 1 + 2 run in float32 only, got %s' % x.dtype)
+    _ffi.require_cuda_real(x, 'x')
+    L = _ffi.lib()
+    f = [_ffi.host_taps(t) for t in (h0o, h1o, h0a, h1a, h0b, h1b)]
+    N, C, H, W = x.shape
+    if H % 4 or W % 4:
+        raise ValueError('the fused DTCWT levels 1 + 2 need a height and width divisible by 4, got {}'.format(tuple(x.shape)))
+    x, xps, xpitch = _ffi.planes_view(x)
+    ll = x.new_empty((N, C, H // 2, W // 2))
+    shape0, hs0 = highs_shape_strides(N, C, H // 2, W // 2, o5, ri)
+    highs0 = x.new_empty(shape0)
+    highs1, hs1 = None, [0] * 6
+    if not skip_hps1:
+        shape1, hs1 = highs_shape_strides(N, C, H // 4, W // 4, o5, ri)
+        highs1 = x.new_empty(shape1)
+    if N * C > 0:
+        if _ffi._USE_GENERIC:
+            ws_bytes = 4 * N * C * H * W
+        else:
+            ws_bytes = L.b200w_dtcwt_fwd_j12_workspace(x.data_ptr(), xps, xpitch, highs0.data_ptr(), N, C, H, W,
+                                                       f[0].n, f[1].n, f[2].n)
+            _ffi.check(ws_bytes if ws_bytes < 0 else 0, 'b200w_dtcwt_fwd_j12_workspace')
+        ws = x.new_empty((ws_bytes // 4,)) if ws_bytes > 0 else None
+        with torch.cuda.device(x.device), _ffi.span('dtcwt_fwd_j12 %dx%d' % (H, W),
+                                                    N * C * H * W * (17 if skip_hps1 else 20)):
+            rc = _ffi.entry('b200w_dtcwt_fwd_j12')(
+                x.data_ptr(), xps, xpitch, ll.data_ptr(), (H // 2) * (W // 2), W // 2,
+                highs0.data_ptr(), _ffi.hs_array(hs0), None if highs1 is None else highs1.data_ptr(), _ffi.hs_array(hs1),
+                N, C, H, W, f[0].p(torch.float32), f[0].n, f[1].p(torch.float32), f[1].n,
+                f[2].p(torch.float32), f[3].p(torch.float32), f[4].p(torch.float32), f[5].p(torch.float32), f[2].n,
+                mode, None if ws is None else ws.data_ptr(), ws_bytes, _ffi.stream_of(x))
+        _ffi.check(rc, 'b200w_dtcwt_fwd_j12')
+    return ll, highs0, highs1
+
+
 def _inv_prepare(ll, highs, o5, ri, what):
     if _is_empty(ll):
         ll = None
@@ -290,6 +329,35 @@ class FWD_J2PLUS(Function):
             # the interpolating filters correlate, so the trees swap (reference :398-401)
             dx = inv_j2plus(dl, None if _is_empty(dh) else dh, h0b, h1b, h0a, h1a, o5, ri)
         return dx, None, None, None, None, None, None, None, None
+
+
+class FWD_J12(Function):
+    """Differentiable levels 1 and 2 of the forward DTCWT in one call, without the level-1 low-pass:
+    ``apply(x, h0o, h1o, h0a, h1a, h0b, h1b, skip_hps1, o_dim, ri_dim, mode)`` -> (ll2, highs0, highs1).
+    Forward and backward equal FWD_J1 followed by FWD_J2PLUS bit for bit (the backward runs the same kernels in the
+    same order: FWD_J2PLUS's backward, then FWD_J1's)."""
+
+    @staticmethod
+    def forward(ctx, x, h0o, h1o, h0a, h1a, h0b, h1b, skip_hps1, o_dim, ri_dim, mode):
+        mode = _mode_int(mode)
+        ctx.mode = mode
+        ctx.taps = tuple(_ffi.host_taps(f) for f in (h0o, h1o, h0a, h1a, h0b, h1b))
+        ctx.dims = get_dimensions5(o_dim, ri_dim)
+        o5, ri = ctx.dims[0], ctx.dims[1]
+        ll, highs0, highs1 = fwd_j12(x, *ctx.taps, bool(skip_hps1), o5, ri, mode)
+        if highs1 is None:
+            highs1 = ll.new_zeros([])
+        return ll, highs0, highs1
+
+    @staticmethod
+    def backward(ctx, dl, dh0, dh1):
+        h0o, h1o, h0a, h1a, h0b, h1b = ctx.taps
+        dx = None
+        if ctx.needs_input_grad[0]:
+            o5, ri = ctx.dims[0], ctx.dims[1]
+            dll1 = inv_j2plus(dl, None if _is_empty(dh1) else dh1, h0b, h1b, h0a, h1a, o5, ri)
+            dx = inv_j1(dll1, None if _is_empty(dh0) else dh0, h0o, h1o, o5, ri, ctx.mode)
+        return dx, None, None, None, None, None, None, None, None, None, None
 
 
 class INV_J1(Function):
