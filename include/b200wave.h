@@ -230,6 +230,41 @@ int b200w_dtcwt1d_inv_j2plus_f64(const double* lo, long long lo_pitch, const dou
                                  void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * 1-D scattering levels (ScatLayer1D / ScatLayer1Dj2): a 1-D DTCWT forward level with the scattering epilogue, one
+ * kernel.  x is N * C rows of length n with row pitch x_pitch >= n.  Element (b, c, i) of an output of row length m is
+ * at base + b * bstride + c * m + i, with bstride >= C * m, so an output can be one slot s of a (N, S, C, m) tensor
+ * (base + s * C * m, bstride S * C * m).  With (re, im) = (hi[2q], hi[2q + 1]) the band-pass pairs of the level and
+ * b = (T)magbias, b2 = (T)(magbias * magbias) (product in double), every operation rounded:
+ *   mag[q] = sqrt((re * re + im * im) + b2) - b;  dre[q] = re / r, dim[q] = im / r, r the rounded root;
+ *   pool(lo)[q] = (lo[2q] + lo[2q + 1]) * 0.5.
+ *   b200w_scat1d_j1:     lo, hi = colfilter(x, h0), colfilter(x, h1), mode symmetric or zero; n even.  Writes
+ *                        pool(lo) (m = n / 2) when pool_lo, else lo itself (m = n); mag (m = n / 2).
+ *   b200w_scat1d_j2plus: lo, hi = coldfilt(x, h0b, h0a), coldfilt(x, h1b, h1a, highpass); n % 4 == 0.  Writes pool(lo)
+ *                        and mag (m = n / 4).
+ *   dre and dim (row length of mag) are both NULL (not written) or both given.
+ * Errors as b200w_dtcwt1d_*: B200W_EARG for a NULL required pointer, only one of dre / dim, a pitch or batch stride
+ * below its row block; B200W_EMODE for a level-1 mode other than zero / symmetric; B200W_ESIZE for negative N or C,
+ * N * C above INT_MAX, n odd (j1) or n % 4 != 0 (j2plus); B200W_EFILTER for a bad filter length.  N * C == 0 returns 0
+ * without a launch.
+ */
+int b200w_scat1d_j1(const float* x, long long x_pitch, int N, int C, int n, float* lo, long long lo_bstride, int pool_lo,
+                    float* mag, long long mag_bstride, float* dre, long long dre_bstride, float* dim,
+                    long long dim_bstride, const float* h0, int L0, const float* h1, int L1, int mode, double magbias,
+                    void* stream);
+int b200w_scat1d_j2plus(const float* x, long long x_pitch, int N, int C, int n, float* lo, long long lo_bstride,
+                        float* mag, long long mag_bstride, float* dre, long long dre_bstride, float* dim,
+                        long long dim_bstride, const float* h0a, const float* h1a, const float* h0b, const float* h1b,
+                        int m, double magbias, void* stream);
+int b200w_scat1d_j1_f64(const double* x, long long x_pitch, int N, int C, int n, double* lo, long long lo_bstride,
+                        int pool_lo, double* mag, long long mag_bstride, double* dre, long long dre_bstride,
+                        double* dim, long long dim_bstride, const double* h0, int L0, const double* h1, int L1,
+                        int mode, double magbias, void* stream);
+int b200w_scat1d_j2plus_f64(const double* x, long long x_pitch, int N, int C, int n, double* lo, long long lo_bstride,
+                            double* mag, long long mag_bstride, double* dre, long long dre_bstride, double* dim,
+                            long long dim_bstride, const double* h0a, const double* h1a, const double* h0b,
+                            const double* h1b, int m, double magbias, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * DTCWT.  "highs" is the reference's 6-D complex band-pass tensor; because o_dim / ri_dim are
  * configurable (dtcwt/transform_funcs.py:10-58) it is described by six ELEMENT strides
  * hs[6] = {n, c, orientation, row, col, real/imag}.  Default layout (N,C,6,H/2,W/2,2) is the

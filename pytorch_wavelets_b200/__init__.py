@@ -3,8 +3,8 @@ fbcotter/pytorch_wavelets, behind the reference's nn.Module API.
 
 The reference package's export list and aliases (``pytorch_wavelets/__init__.py:1-36``) for the classes on the
 hot path and its direct callers (SURVEY.md section 8), plus the 3-D DWT (``DWT3DForward`` / ``DWT3DInverse``,
-aliases ``DWT3D`` / ``IDWT3D``) and the 1-D DTCWT (``DTCWT1DForward`` / ``DTCWT1DInverse``, aliases ``DTCWT1D`` /
-``IDTCWT1D``), which the reference does not have.
+aliases ``DWT3D`` / ``IDWT3D``), the 1-D DTCWT (``DTCWT1DForward`` / ``DTCWT1DInverse``, aliases ``DTCWT1D`` /
+``IDTCWT1D``) and the 1-D scattering layers (``ScatLayer1D`` / ``ScatLayer1Dj2``), which the reference does not have.
 Every transform runs in hand-written CUDA kernels through the C ABI of ``libb200wave.so``; there is no
 CPU or eager fallback.
 """
@@ -34,6 +34,8 @@ __all__ = [
     'IDWT3D',
     'ScatLayer',
     'ScatLayerj2',
+    'ScatLayer1D',
+    'ScatLayer1Dj2',
 ]
 
 from pytorch_wavelets_b200._version import __version__
@@ -42,7 +44,7 @@ from pytorch_wavelets_b200.dtcwt.transform2d import DTCWTForward, DTCWTInverse
 from pytorch_wavelets_b200.dwt.transform1d import DWT1DForward, DWT1DInverse
 from pytorch_wavelets_b200.dwt.transform2d import DWTForward, DWTInverse
 from pytorch_wavelets_b200.dwt.transform3d import DWT3DForward, DWT3DInverse
-from pytorch_wavelets_b200.scatternet import ScatLayer, ScatLayerj2
+from pytorch_wavelets_b200.scatternet import ScatLayer, ScatLayer1D, ScatLayer1Dj2, ScatLayerj2
 
 # aliases, as in the reference
 DTCWT = DTCWTForward

@@ -36,7 +36,8 @@ SYMBOLS = SYMBOLS + [s + '_generic' for s in KERNEL_ENTRIES] + [s + '_f64' for s
     'b200w_dtcwt_ifilt_f64'] + [
     'b200w_dwt_%s3d%s%s' % (d, w, v) for d in ('afb', 'sfb') for w in ('', '_workspace') for v in ('', '_generic', '_f64')] + [
     'b200w_dtcwt1d_%s%s' % (k, v) for k in ('fwd_j1', 'fwd_j2plus', 'inv_j1', 'inv_j2plus') for v in ('', '_f64')] + [
-    'b200w_dtcwt_fwd_j12', 'b200w_dtcwt_fwd_j12_generic', 'b200w_dtcwt_fwd_j12_workspace']
+    'b200w_dtcwt_fwd_j12', 'b200w_dtcwt_fwd_j12_generic', 'b200w_dtcwt_fwd_j12_workspace'] + [
+    'b200w_scat1d_%s%s' % (k, v) for k in ('j1', 'j2plus') for v in ('', '_f64')]
 
 
 class B200WaveError(RuntimeError):
@@ -104,6 +105,13 @@ def lib():
                                                                c_int, c_vp]
             getattr(L, 'b200w_dtcwt1d_inv_j2plus' + v).argtypes = [c_vp, c_ll, c_vp, c_int, c_int, c_vp, pf, pf, pf, pf,
                                                                    c_int, c_vp]
+            # 1-D scattering levels: x, pitch, N, C, n, then (pointer, batch stride) of each output
+            getattr(L, 'b200w_scat1d_j1' + v).argtypes = [c_vp, c_ll, c_int, c_int, c_int, c_vp, c_ll, c_int, c_vp, c_ll,
+                                                          c_vp, c_ll, c_vp, c_ll, pf, c_int, pf, c_int, c_int,
+                                                          ctypes.c_double, c_vp]
+            getattr(L, 'b200w_scat1d_j2plus' + v).argtypes = [c_vp, c_ll, c_int, c_int, c_int, c_vp, c_ll, c_vp, c_ll,
+                                                              c_vp, c_ll, c_vp, c_ll, pf, pf, pf, pf, c_int,
+                                                              ctypes.c_double, c_vp]
         for v in ('', '_generic'):   # DTCWT forward levels 1 + 2 (csrc/dtcwt_fwd12.cuh)
             getattr(L, 'b200w_dtcwt_fwd_j12' + v).argtypes = [c_vp, c_ll, c_int, c_vp, c_ll, c_int, c_vp, hs, c_vp, hs,
                                                               c_int, c_int, c_int, c_int, pf, c_int, pf, c_int,

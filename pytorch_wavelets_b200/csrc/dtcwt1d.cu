@@ -16,6 +16,9 @@
 // Consecutive threads take consecutive units, so every warp stores contiguous runs.  Accumulation is the oracle's and
 // k_prims.cu's: a product, then fused multiply-adds in stored-tap order; the inverses round each branch and add them
 // with add_rn, so the results are bit-identical to the oracle primitives in both precisions.
+// k_scat1d runs FWD1 / FWD2 with the scattering epilogue of ScatLayer1D / ScatLayer1Dj2 (pooled low-pass, smoothed
+// magnitude of each (re, im) band-pass pair, optionally its derivatives) on the same body, so its filter outputs are
+// those of k_dt1d; k_dt1d itself compiles to the same code as without the epilogue.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -30,9 +33,13 @@ enum Kind { FWD1 = 0, FWD2 = 1, INV1 = 2, INV2 = 3 };
 constexpr int kThreads = 256;
 constexpr int kPackSmem = 48 * 1024;   // staging budget of a packed CTA
 
+// Scattering epilogue of the forward kernels (k_scat1d): SC = 0 none, SC_MAG smoothed magnitude, SC_DER magnitude and
+// its derivatives.  A level-1 unit is then one output pair (x[2q], x[2q + 1]) of each filter.
+enum Scat { SC_NONE = 0, SC_MAG = 1, SC_DER = 2 };
+
 // input samples per unit, staged inputs, units per long-row segment (2048 input samples of each input)
-template <int K> struct KindInfo {
-  static constexpr int ipu = K == FWD2 ? 4 : (K == INV2 ? 2 : 1);
+template <int K, int SC = SC_NONE> struct KindInfo {
+  static constexpr int ipu = K == FWD2 ? 4 : (K == INV2 || (K == FWD1 && SC != SC_NONE) ? 2 : 1);
   static constexpr int nin = (K == INV1 || K == INV2) ? 2 : 1;
   static constexpr int seg = 2048 / ipu;
 };
@@ -50,6 +57,17 @@ struct Dt1dParams {
   // level 1: a0 = branch-0 filter (h0 / g0), a1 = branch-1 filter (h1 / g1);
   // levels >= 2: (ha, hb) of the coldfilt / colifilt call of branch 0 (low-pass) and branch 1 (high-pass)
   TapsT<T> a0, b0, a1, b1;
+};
+
+// The scattering forms append their outputs, so the plain kernels' parameter layout is the one above.  Row r = b * C + c
+// of an output of row length m (= units) is at base + b * bstride + c * m: out0 = low-pass (2x pooled, or at level 1
+// the full-length low-pass when !pool), mag = sqrt(re^2 + im^2 + b^2) - b, dre / dim = re / r, im / r (SC_DER).
+template <class T>
+struct Scat1dParams : Dt1dParams<T> {
+  T* mag; T* dre; T* dim;
+  long long bs_lo, bs_mag, bs_dre, bs_dim;
+  int C, pool;
+  T magbias, magbias2;              // b and T(b * b), the product in double
 };
 
 __device__ __forceinline__ void cp_async16(void* sdst, const void* gsrc) {
@@ -99,10 +117,31 @@ __device__ __forceinline__ T sum2(bool h0, T a, bool h1, T b) {
   return h0 ? (h1 ? add_rn(a, b) : a) : (h1 ? b : (T)0);
 }
 
-// LA, LB: level-1 filter lengths (branch 0, branch 1); levels >= 2: LA = m.  0 = runtime length.
-template <class T, int K, int LA, int LB, bool PACK>
-__global__ void __launch_bounds__(kThreads) k_dt1d(const __grid_constant__ Dt1dParams<T> p) {
-  using KI = KindInfo<K>;
+// One (lo, hi) output pair of a forward level into the scattering outputs of row `row`, position q.
+template <int SC, class T>
+__device__ __forceinline__ void scat_store(const Scat1dParams<T>& p, int row, int q, T lo0, T lo1, T re, T im) {
+  const int b = row / p.C, c = row - b * p.C;
+  const long long o = (long long)c * p.units + q;
+  if (p.pool) {
+    p.out0[b * p.bs_lo + o] = mul_rn(add_rn(lo0, lo1), (T)0.5);
+  } else {
+    const long long ol = b * p.bs_lo + 2 * o;
+    p.out0[ol] = lo0;
+    p.out0[ol + 1] = lo1;
+  }
+  const T r = sqrt_rn(add_rn(add_rn(mul_rn(re, re), mul_rn(im, im)), p.magbias2));
+  p.mag[b * p.bs_mag + o] = sub_rn(r, p.magbias);
+  if (SC == SC_DER) {
+    p.dre[b * p.bs_dre + o] = div_rn(re, r);
+    p.dim[b * p.bs_dim + o] = div_rn(im, r);
+  }
+}
+
+// The body of every level kernel.  LA, LB: level-1 filter lengths (branch 0, branch 1); levels >= 2: LA = m.
+// 0 = runtime length.  P is Dt1dParams<T>, or Scat1dParams<T> when SC != SC_NONE.
+template <class T, int K, int LA, int LB, bool PACK, int SC, class P>
+__device__ __forceinline__ void dt1d_body(const P& p) {
+  using KI = KindInfo<K, SC>;
   constexpr int VEC = 16 / (int)sizeof(T);
   extern __shared__ __align__(16) unsigned char smem_raw[];
   T* smem = reinterpret_cast<T*>(smem_raw);
@@ -163,7 +202,23 @@ __global__ void __launch_bounds__(kThreads) k_dt1d(const __grid_constant__ Dt1dP
       s0 = smem + (size_t)r * p.srow + ((misalign(p.in0 + (long long)row * p.pitch0) + g0) & (VEC - 1));
     if (KI::nin == 2 && p.in1)
       s1 = smem + (size_t)(p.rpc + r) * p.srow + ((misalign(p.in1 + (long long)row * p.nin) + g0) & (VEC - 1));
-    if (K == FWD1) {
+    if constexpr (SC != SC_NONE) {
+      // the filter outputs of the FWD1 / FWD2 branches below, one output pair of each filter per unit
+      const int q = u0 + u;
+      if (K == FWD1) {
+        const int w = 2 * u + p.halo;
+        const int l0 = LA > 0 ? LA : p.L0, l1 = LB > 0 ? LB : p.L1;
+        const T* xa = s0 + w - l0 / 2;
+        const T* xb = s0 + w - l1 / 2;
+        scat_store<SC>(p, row, q, corr<LA, 1, 1>(p.a0.t, xa, l0), corr<LA, 1, 1>(p.a0.t, xa + 1, l0),
+                       corr<LB, 1, 1>(p.a1.t, xb, l1), corr<LB, 1, 1>(p.a1.t, xb + 1, l1));
+      } else {   // FWD2
+        const int m = LA > 0 ? LA : p.L0;
+        const T* xa = s0 + 4 * u + 2;
+        scat_store<SC>(p, row, q, corr<LA, 1, 2>(p.a0.t, xa, m), corr<LA, 1, 2>(p.b0.t, xa + 1, m),
+                       corr<LA, 1, 2>(p.b1.t, xa + 1, m), corr<LA, 1, 2>(p.a1.t, xa, m));
+      }
+    } else if (K == FWD1) {
       const int i = u0 + u, w = u + p.halo;
       const int l0 = LA > 0 ? LA : p.L0, l1 = LB > 0 ? LB : p.L1;
       p.out0[(long long)row * p.nout + i] = corr<LA, 1, 1>(p.a0.t, s0 + w - l0 / 2, l0);
@@ -199,6 +254,17 @@ __global__ void __launch_bounds__(kThreads) k_dt1d(const __grid_constant__ Dt1dP
   }
 }
 
+template <class T, int K, int LA, int LB, bool PACK>
+__global__ void __launch_bounds__(kThreads) k_dt1d(const __grid_constant__ Dt1dParams<T> p) {
+  dt1d_body<T, K, LA, LB, PACK, SC_NONE>(p);
+}
+
+// K = FWD1 or FWD2 with the scattering epilogue
+template <class T, int K, int LA, int LB, bool PACK, int SC>
+__global__ void __launch_bounds__(kThreads) k_scat1d(const __grid_constant__ Scat1dParams<T> p) {
+  dt1d_body<T, K, LA, LB, PACK, SC>(p);
+}
+
 // ---- host side -------------------------------------------------------------------------------------------------
 
 template <class T>
@@ -206,9 +272,15 @@ static void set_taps(TapsT<T>& d, const T* src, int L) {
   for (int i = 0; i < kMaxTaps; ++i) d.t[i] = (i < L) ? src[i] : (T)0;
 }
 
-template <class T, int K, int LA, int LB>
-static int launch_kind(Dt1dParams<T>& p, void* stream) {
-  using KI = KindInfo<K>;
+template <class T, int K, int LA, int LB, bool PACK, int SC>
+static auto kernel_of() {
+  if constexpr (SC == SC_NONE) return k_dt1d<T, K, LA, LB, PACK>;
+  else return k_scat1d<T, K, LA, LB, PACK, SC>;
+}
+
+template <class T, int K, int LA, int LB, int SC, class P>
+static int launch_kind(P& p, void* stream) {
+  using KI = KindInfo<K, SC>;
   constexpr int VEC = 16 / (int)sizeof(T);
   auto srow_of = [&](int units) { return ((units * KI::ipu + 2 * p.halo + 2 * VEC - 1) / VEC) * VEC; };
   // packed CTA: at least two whole rows within KindInfo::seg units and the staging budget
@@ -218,37 +290,38 @@ static int launch_kind(Dt1dParams<T>& p, void* stream) {
   if (rpc >= 2) {
     p.seg = p.units; p.rpc = rpc; p.nseg = 1; p.srow = srow;
     const long long blocks = (p.rows + rpc - 1) / rpc;
-    return launch(k_dt1d<T, K, LA, LB, true>, p, blocks, kThreads, (size_t)KI::nin * rpc * srow * sizeof(T), stream);
+    return launch(kernel_of<T, K, LA, LB, true, SC>(), p, blocks, kThreads, (size_t)KI::nin * rpc * srow * sizeof(T),
+                  stream);
   }
   p.seg = KI::seg; p.rpc = 1; p.nseg = (p.units + KI::seg - 1) / KI::seg; p.srow = srow_of(imin(p.units, KI::seg));
   const long long blocks = (long long)p.rows * p.nseg;
   if (blocks > 2147483647LL) return B200W_ESIZE;
-  return launch(k_dt1d<T, K, LA, LB, false>, p, blocks, kThreads, (size_t)KI::nin * p.srow * sizeof(T), stream);
+  return launch(kernel_of<T, K, LA, LB, false, SC>(), p, blocks, kThreads, (size_t)KI::nin * p.srow * sizeof(T), stream);
 }
 
 // level 1: the (L0, L1) pairs of the biorthogonal tables, in both orders (the backward passes swap directions)
-template <class T, int K>
-static int dispatch_j1(Dt1dParams<T>& p, void* stream) {
+template <class T, int K, int SC = SC_NONE, class P>
+static int dispatch_j1(P& p, void* stream) {
   const int a = p.L0, b = p.L1;
-#define B200W_DT1D_PAIR(X, Y) if (a == X && b == Y) return launch_kind<T, K, X, Y>(p, stream);
+#define B200W_DT1D_PAIR(X, Y) if (a == X && b == Y) return launch_kind<T, K, X, Y, SC>(p, stream);
   B200W_DT1D_PAIR(5, 7) B200W_DT1D_PAIR(7, 5)      // near_sym_a
   B200W_DT1D_PAIR(9, 7) B200W_DT1D_PAIR(7, 9)      // antonini
   B200W_DT1D_PAIR(5, 3) B200W_DT1D_PAIR(3, 5)      // legall
   B200W_DT1D_PAIR(13, 19) B200W_DT1D_PAIR(19, 13)  // near_sym_b
 #undef B200W_DT1D_PAIR
-  return launch_kind<T, K, 0, 0>(p, stream);
+  return launch_kind<T, K, 0, 0, SC>(p, stream);
 }
 
 // levels >= 2: the q-shift table lengths
-template <class T, int K>
-static int dispatch_j2(Dt1dParams<T>& p, void* stream) {
+template <class T, int K, int SC = SC_NONE, class P>
+static int dispatch_j2(P& p, void* stream) {
   switch (p.L0) {
-    case 10: return launch_kind<T, K, 10, 0>(p, stream);   // qshift_06, qshift_a
-    case 14: return launch_kind<T, K, 14, 0>(p, stream);   // qshift_b
-    case 16: return launch_kind<T, K, 16, 0>(p, stream);   // qshift_c
-    case 18: return launch_kind<T, K, 18, 0>(p, stream);   // qshift_d
-    case 32: return launch_kind<T, K, 32, 0>(p, stream);   // qshift_32
-    default: return launch_kind<T, K, 0, 0>(p, stream);
+    case 10: return launch_kind<T, K, 10, 0, SC>(p, stream);   // qshift_06, qshift_a
+    case 14: return launch_kind<T, K, 14, 0, SC>(p, stream);   // qshift_b
+    case 16: return launch_kind<T, K, 16, 0, SC>(p, stream);   // qshift_c
+    case 18: return launch_kind<T, K, 18, 0, SC>(p, stream);   // qshift_d
+    case 32: return launch_kind<T, K, 32, 0, SC>(p, stream);   // qshift_32
+    default: return launch_kind<T, K, 0, 0, SC>(p, stream);
   }
 }
 
@@ -323,6 +396,61 @@ static int inv_j2(const T* lo, long long pitch, const T* hi, int rows, int n, T*
   return dispatch_j2<T, INV2>(p, stream);
 }
 
+// Shared argument checks and output fields of the scattering entries; m = output row length.  Returns 1 when there is
+// a launch to make, else B200W_OK or an error code.
+template <class T>
+static int scat_setup(Scat1dParams<T>& p, const T* x, long long pitch, int N, int C, int n, T* lo, long long bs_lo,
+                      int m_lo, T* mag, long long bs_mag, T* dre, long long bs_dre, T* dim, long long bs_dim, int m,
+                      double magbias) {
+  if (!x || !lo || !mag || (!dre != !dim)) return B200W_EARG;
+  if (N < 0 || C < 0 || (long long)N * C > 2147483647LL) return B200W_ESIZE;
+  const long long cm = (long long)C * m;
+  if (pitch < n || bs_lo < (long long)C * m_lo || bs_mag < cm || (dre && (bs_dre < cm || bs_dim < cm)))
+    return B200W_EARG;
+  p.rows = N * C; p.nin = n; p.units = m;
+  p.in0 = x; p.pitch0 = pitch; p.in1 = nullptr; p.out0 = lo; p.out1 = nullptr;
+  p.mag = mag; p.dre = dre; p.dim = dim;
+  p.bs_lo = bs_lo; p.bs_mag = bs_mag; p.bs_dre = bs_dre; p.bs_dim = bs_dim;
+  p.C = C; p.pool = m_lo == m;
+  p.magbias = (T)magbias; p.magbias2 = (T)(magbias * magbias);
+  return 1;
+}
+
+template <class T>
+static int scat_j1(const T* x, long long pitch, int N, int C, int n, T* lo, long long bs_lo, int pool, T* mag,
+                   long long bs_mag, T* dre, long long bs_dre, T* dim, long long bs_dim, const T* h0, int L0,
+                   const T* h1, int L1, int mode, double magbias, void* stream) {
+  if (mode != B200W_MODE_SYMMETRIC && mode != B200W_MODE_ZERO) return B200W_EMODE;
+  if (!h0 || !h1) return B200W_EARG;
+  if (n < 2 || (n & 1)) return B200W_ESIZE;
+  Scat1dParams<T> p = {};
+  const int rc = scat_setup(p, x, pitch, N, C, n, lo, bs_lo, pool ? n / 2 : n, mag, bs_mag, dre, bs_dre, dim, bs_dim,
+                            n / 2, magbias);
+  if (rc <= 0) return rc;
+  if (!l1_ok(L0) || !l1_ok(L1)) return B200W_EFILTER;
+  if (p.rows == 0) return B200W_OK;
+  p.L0 = L0; p.L1 = L1; p.halo = imax(L0, L1) / 2; p.sym = mode == B200W_MODE_SYMMETRIC;
+  set_taps(p.a0, h0, L0); set_taps(p.a1, h1, L1);
+  return dre ? dispatch_j1<T, FWD1, SC_DER>(p, stream) : dispatch_j1<T, FWD1, SC_MAG>(p, stream);
+}
+
+template <class T>
+static int scat_j2(const T* x, long long pitch, int N, int C, int n, T* lo, long long bs_lo, T* mag, long long bs_mag,
+                   T* dre, long long bs_dre, T* dim, long long bs_dim, const T* h0a, const T* h1a, const T* h0b,
+                   const T* h1b, int m, double magbias, void* stream) {
+  if (!h0a || !h1a || !h0b || !h1b) return B200W_EARG;
+  if (n < 4 || (n % 4)) return B200W_ESIZE;
+  Scat1dParams<T> p = {};
+  const int rc = scat_setup(p, x, pitch, N, C, n, lo, bs_lo, n / 4, mag, bs_mag, dre, bs_dre, dim, bs_dim, n / 4,
+                            magbias);
+  if (rc <= 0) return rc;
+  if (!qs_ok(m)) return B200W_EFILTER;
+  if (p.rows == 0) return B200W_OK;
+  p.L0 = m; p.L1 = m; p.halo = m; p.sym = 1;
+  set_taps(p.a0, h0b, m); set_taps(p.b0, h0a, m); set_taps(p.a1, h1b, m); set_taps(p.b1, h1a, m);
+  return dre ? dispatch_j2<T, FWD2, SC_DER>(p, stream) : dispatch_j2<T, FWD2, SC_MAG>(p, stream);
+}
+
 }  // namespace dt1d
 }  // namespace b200w
 
@@ -365,6 +493,35 @@ int b200w_dtcwt1d_inv_j2plus_f64(const double* lo, long long lo_pitch, const dou
                                  const double* g0a, const double* g1a, const double* g0b, const double* g1b, int m,
                                  void* stream) {
   return inv_j2<double>(lo, lo_pitch, hi, rows, n, y, g0a, g1a, g0b, g1b, m, stream);
+}
+
+int b200w_scat1d_j1(const float* x, long long x_pitch, int N, int C, int n, float* lo, long long lo_bstride, int pool_lo,
+                    float* mag, long long mag_bstride, float* dre, long long dre_bstride, float* dim,
+                    long long dim_bstride, const float* h0, int L0, const float* h1, int L1, int mode, double magbias,
+                    void* stream) {
+  return scat_j1<float>(x, x_pitch, N, C, n, lo, lo_bstride, pool_lo, mag, mag_bstride, dre, dre_bstride, dim,
+                        dim_bstride, h0, L0, h1, L1, mode, magbias, stream);
+}
+int b200w_scat1d_j1_f64(const double* x, long long x_pitch, int N, int C, int n, double* lo, long long lo_bstride,
+                        int pool_lo, double* mag, long long mag_bstride, double* dre, long long dre_bstride,
+                        double* dim, long long dim_bstride, const double* h0, int L0, const double* h1, int L1,
+                        int mode, double magbias, void* stream) {
+  return scat_j1<double>(x, x_pitch, N, C, n, lo, lo_bstride, pool_lo, mag, mag_bstride, dre, dre_bstride, dim,
+                         dim_bstride, h0, L0, h1, L1, mode, magbias, stream);
+}
+int b200w_scat1d_j2plus(const float* x, long long x_pitch, int N, int C, int n, float* lo, long long lo_bstride,
+                        float* mag, long long mag_bstride, float* dre, long long dre_bstride, float* dim,
+                        long long dim_bstride, const float* h0a, const float* h1a, const float* h0b, const float* h1b,
+                        int m, double magbias, void* stream) {
+  return scat_j2<float>(x, x_pitch, N, C, n, lo, lo_bstride, mag, mag_bstride, dre, dre_bstride, dim, dim_bstride,
+                        h0a, h1a, h0b, h1b, m, magbias, stream);
+}
+int b200w_scat1d_j2plus_f64(const double* x, long long x_pitch, int N, int C, int n, double* lo, long long lo_bstride,
+                            double* mag, long long mag_bstride, double* dre, long long dre_bstride, double* dim,
+                            long long dim_bstride, const double* h0a, const double* h1a, const double* h0b,
+                            const double* h1b, int m, double magbias, void* stream) {
+  return scat_j2<double>(x, x_pitch, N, C, n, lo, lo_bstride, mag, mag_bstride, dre, dre_bstride, dim, dim_bstride,
+                         h0a, h1a, h0b, h1b, m, magbias, stream);
 }
 
 }  // extern "C"
