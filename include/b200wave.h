@@ -265,6 +265,41 @@ int b200w_scat1d_j2plus_f64(const double* x, long long x_pitch, int N, int C, in
                             const double* h1b, int m, double magbias, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * 2-D wavelet packet levels (csrc/wpt2d.cu).  One DWT analysis / synthesis level (the arithmetic of
+ * b200w_dwt_afb2d / b200w_dwt_sfb2d) applied to every plane, in the packet layout: the four children
+ * of plane p (ll, lh, hl, hh) are nodes 4p .. 4p+3, so one level's output is the next level's input.
+ *   b200w_wpt_afb2d: x planes (plane stride, row pitch) -> node 4p + b at y + (4p + b) * y_node_stride,
+ *                    rows y_pitch apart; Ho, Wo = b200w_dwt_coeff_len of H, W.
+ *   b200w_wpt_sfb2d: c contiguous (planes * 4, Hc, Wc) -> y planes (plane stride, row pitch) of Ho x Wo,
+ *                    Ho / Wo at most b200w_dwt_rec_len of Hc / Wc (smaller values crop, as in the
+ *                    analysis backward pass).
+ * The route is chosen per call from the plane size, filter lengths and alignment: a packed small-plane
+ * kernel, the streaming kernel (float32, Lw == Lh <= 20) or the generic tile kernel (every case; the
+ * only one the _generic entries run).  Errors: B200W_EMODE for an unknown mode; B200W_EARG for a NULL
+ * pointer, a pitch below its row length, or a node / plane stride below Ho * pitch; B200W_ESIZE for bad
+ * sizes or a grid that is too large; B200W_EFILTER for a length outside 2 .. B200W_MAX_TAPS (Lw != Lh is
+ * allowed).  planes == 0 returns 0 without a launch.
+ */
+int b200w_wpt_afb2d(const float* x, long long x_plane_stride, int x_pitch, float* y, long long y_node_stride,
+                    int y_pitch, int planes, int H, int W, const float* fw_lo, const float* fw_hi, int Lw,
+                    const float* fh_lo, const float* fh_hi, int Lh, int mode, void* stream);
+int b200w_wpt_afb2d_generic(const float* x, long long x_plane_stride, int x_pitch, float* y, long long y_node_stride,
+                            int y_pitch, int planes, int H, int W, const float* fw_lo, const float* fw_hi, int Lw,
+                            const float* fh_lo, const float* fh_hi, int Lh, int mode, void* stream);
+int b200w_wpt_afb2d_f64(const double* x, long long x_plane_stride, int x_pitch, double* y, long long y_node_stride,
+                        int y_pitch, int planes, int H, int W, const double* fw_lo, const double* fw_hi, int Lw,
+                        const double* fh_lo, const double* fh_hi, int Lh, int mode, void* stream);
+int b200w_wpt_sfb2d(const float* c, float* y, long long y_plane_stride, int y_pitch, int planes, int Hc, int Wc,
+                    int Ho, int Wo, const float* gh_lo, const float* gh_hi, int Lh, const float* gw_lo,
+                    const float* gw_hi, int Lw, int mode, void* stream);
+int b200w_wpt_sfb2d_generic(const float* c, float* y, long long y_plane_stride, int y_pitch, int planes, int Hc,
+                            int Wc, int Ho, int Wo, const float* gh_lo, const float* gh_hi, int Lh, const float* gw_lo,
+                            const float* gw_hi, int Lw, int mode, void* stream);
+int b200w_wpt_sfb2d_f64(const double* c, double* y, long long y_plane_stride, int y_pitch, int planes, int Hc, int Wc,
+                        int Ho, int Wo, const double* gh_lo, const double* gh_hi, int Lh, const double* gw_lo,
+                        const double* gw_hi, int Lw, int mode, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * DTCWT.  "highs" is the reference's 6-D complex band-pass tensor; because o_dim / ri_dim are
  * configurable (dtcwt/transform_funcs.py:10-58) it is described by six ELEMENT strides
  * hs[6] = {n, c, orientation, row, col, real/imag}.  Default layout (N,C,6,H/2,W/2,2) is the

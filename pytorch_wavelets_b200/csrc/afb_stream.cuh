@@ -152,73 +152,34 @@ __device__ __forceinline__ void afb_stage_dispatch(int vv, const AfbParams& p, c
   }
 }
 
-// strip0 / n_strips: the 64-column strips this launch covers (PW == 32), or the single remainder strip
-// starting at output column k_rem (PW < 32, n_strips == 1).
-template <int L, int PW, int MINB, int HSM, int XM>
-__global__ void __launch_bounds__(32, (MINB > 1 ? MINB : 0)) afb2d_stream(const __grid_constant__ AfbParams p, int n_strips, int n_chunks,
-                                                   int CH, int k_rem, int swid) {
-  using C = AfbCfg<L, PW, HSM, XM>;
-  extern __shared__ __align__(16) float ring[];  // this warp's staging ring
-  const int lane = threadIdx.x;
-  long long item = blockIdx.x;                    // one warp per CTA: no intra-CTA load imbalance
-  const int strip = (int)(item % n_strips);
-  item /= n_strips;
-  const int chunk = (int)(item % n_chunks);
-  const int pgroup = (int)(item / n_chunks);
-  const int g = lane / PW, jp = lane % PW;        // plane within the group, column pair within the plane
-  const int plane0 = pgroup * C::G;
-  const int nplanes = imin(C::G, p.planes - plane0);
-  const int plane = plane0 + g;
+#define B200W_AFB_KERNEL afb2d_stream
+#define B200W_PK 0
+#include "afb_stream_kernel.cuh"
+#undef B200W_AFB_KERNEL
+#undef B200W_PK
+#define B200W_AFB_KERNEL wpt_afb2d_stream
+#define B200W_PK 1
+#include "afb_stream_kernel.cuh"
+#undef B200W_AFB_KERNEL
+#undef B200W_PK
 
-  // swid = output columns per strip (even, <= 64)
-  const int k0 = (PW == 32) ? strip * swid : k_rem;
-  const int ky0 = chunk * CH;
-  const int ky1 = imin(ky0 + CH, p.Ho);
-  const int n_half = (ky1 - ky0) + C::PRO;             // half-stages: PRO of warm-up, then one output row each
-  const int n_stage = (n_half + C::HS - 1) / C::HS;
-  const int nvalid = imin((PW == 32) ? swid : 2 * PW, p.Wo - k0);
-
-  const int sh = (XM == 0 && PW == 32) ? widen_left(2 * k0 - C::HLA, C::HLA + 2 * nvalid + C::RH, p.W, p.mode,
-                                                         C::SW - 4 * C::NV - 4 * ((nvalid + 1) / 2 - 1)) : 0;
-  typename C::Loader ld;
-  ld.init(ring, p.x + (long long)plane0 * p.xps, p.xps, nplanes, p.H, p.W, p.xpitch, p.mode, 2 * k0 - C::HLA - sh,
-          C::HLA + 2 * nvalid + C::RH + sh, 2 * ky0 - C::PL, n_stage, lane);
-  ld.prologue();
-
-  float2 w[L][2];
-#pragma unroll
-  for (int j = 0; j < L; ++j) { w[j][0] = w[j][1] = make_float2(0.f, 0.f); }
-
-  DirectOut out;
-  const int hipitch = p.hipitch > 0 ? p.hipitch : p.Wo;
-  out.band = (long long)p.Ho * hipitch;
-  out.ll_ptr = p.ll + (long long)plane * p.llps + (long long)ky0 * p.llpitch + k0 + 2 * jp;
-  out.hi_ptr = p.highs + (long long)plane * 3 * out.band + (long long)ky0 * hipitch + k0 + 2 * jp;
-  out.nv = (g < nplanes) ? imax(0, imin(2, k0 + nvalid - (k0 + 2 * jp))) : 0;
-  out.llpitch = p.llpitch;
-  out.Wo = hipitch;
-  out.init_parity();
-  const int lane_off = g * (C::RPS * C::SW) + ((sh > 0 && out.nv == 0) ? 0 : 4 * jp + sh);
-
-  int vv = 0;
-#pragma unroll 1
-  for (int t = 0; t < n_stage; ++t) {
-    const float* stage = ld.acquire(t);
-    ld.issue(t + C::NS - 1);
-    afb_stage_dispatch<L, PW, HSM, XM, 0>(vv, p, stage + lane_off, w, C::HS * t, n_half, out);
-    vv = (vv + 1 == C::UNS) ? 0 : vv + 1;
-  }
-  cp_async_wait<0>();
+template <int L, int PW, int MINB, int HSM, bool PK>
+constexpr auto afb_kernel_of() {
+  if constexpr (PK) return wpt_afb2d_stream<L, PW, MINB, HSM, 0>;
+  else return afb2d_stream<L, PW, MINB, HSM, 0>;
 }
 
-template <int L, int PW, int MINB, int HSM, int XM = 0>
+template <int L, int PW, int MINB, int HSM, int XM = 0, bool PK = false>
 inline void launch_afb_kernel(const AfbParams& p, cudaStream_t stream, long long blocks, int n_strips, int n_chunks,
                               int CH, int k_rem) {
   using C = AfbCfg<L, PW, HSM, XM>;
   // strips are 64 columns wide; splitting the columns evenly over the strips instead (g_tune_balanced) gives more row
   // segments that straddle 128-byte lines
   const int swid = 64;
-  afb2d_stream<L, PW, MINB, HSM, XM><<<(unsigned)blocks, 32, C::SMEM_BYTES, stream>>>(p, n_strips, n_chunks, CH, k_rem, swid);
+  if constexpr (PK)
+    wpt_afb2d_stream<L, PW, MINB, HSM, XM><<<(unsigned)blocks, 32, C::SMEM_BYTES, stream>>>(p, n_strips, n_chunks, CH, k_rem, swid);
+  else
+    afb2d_stream<L, PW, MINB, HSM, XM><<<(unsigned)blocks, 32, C::SMEM_BYTES, stream>>>(p, n_strips, n_chunks, CH, k_rem, swid);
 }
 
 #ifndef B200W_AFB_SHORT_MINB
@@ -228,33 +189,33 @@ inline void launch_afb_kernel(const AfbParams& p, cudaStream_t stream, long long
 #define B200W_AFB_LONG_MINB 12  /* resident one-warp CTAs per SM the >= 14-tap instantiations are compiled for
                                   * (a register cap that does not spill; 16 spills) */
 #endif
-template <int L, int PW>
+template <int L, int PW, bool PK = false>
 inline int launch_afb_part(const AfbParams& p, cudaStream_t stream, int n_strips, int k_rem) {
   constexpr int G = 32 / PW;
   const long long groups = ((long long)p.planes + G - 1) / G;
   int n_chunks, CH;
   static ConcCache conc_cache;
-  const int conc = resident_warps_dev(conc_cache, afb2d_stream<L, PW, (L >= 14 ? B200W_AFB_LONG_MINB : B200W_AFB_SHORT_MINB), 2, 0>,
+  const int conc = resident_warps_dev(conc_cache, afb_kernel_of<L, PW, (L >= 14 ? B200W_AFB_LONG_MINB : B200W_AFB_SHORT_MINB), 2, PK>(),
                                       AfbCfg<L, PW, 2, 0>::SMEM_BYTES);
   pick_chunks(groups * n_strips, p.Ho, 16, (L - 2) / 2 + 8, conc, &n_chunks, &CH);
   const long long blocks = groups * n_strips * n_chunks;
   if (blocks <= 0) return 0;
   if (blocks > 2147483647LL) return B200W_ESIZE;
   if (p.mode == B200W_MODE_PERIODIZATION) {
-    launch_afb_kernel<L, PW, 1, 2, 2>(p, stream, blocks, n_strips, n_chunks, CH, k_rem);
+    launch_afb_kernel<L, PW, 1, 2, 2, PK>(p, stream, blocks, n_strips, n_chunks, CH, k_rem);
     return 0;
   }
   if (p.mode == B200W_MODE_PERIODIC) {
-    launch_afb_kernel<L, PW, 1, 2, 1>(p, stream, blocks, n_strips, n_chunks, CH, k_rem);
+    launch_afb_kernel<L, PW, 1, 2, 1, PK>(p, stream, blocks, n_strips, n_chunks, CH, k_rem);
     return 0;
   }
   // tried and not kept: register caps (__launch_bounds__(32, 18..32): faster on the small levels only, slower on the
   // large one) and 8-row stages
-  launch_afb_kernel<L, PW, (L >= 14 ? B200W_AFB_LONG_MINB : B200W_AFB_SHORT_MINB), 2>(p, stream, blocks, n_strips, n_chunks, CH, k_rem);
+  launch_afb_kernel<L, PW, (L >= 14 ? B200W_AFB_LONG_MINB : B200W_AFB_SHORT_MINB), 2, 0, PK>(p, stream, blocks, n_strips, n_chunks, CH, k_rem);
   return 0;
 }
 
-template <int L>
+template <int L, bool PK = false>
 inline int launch_afb_stream(const AfbParams& p, cudaStream_t stream) {
   // aligned 16-byte staging needs an aligned source; anything else takes the generic kernel
   if (!aligned_plane(p.x, p.xps, p.xpitch)) return kNoFastPath;
@@ -262,26 +223,28 @@ inline int launch_afb_stream(const AfbParams& p, cudaStream_t stream) {
   // latency/occupancy-bound, not issue-bound, so a mostly-idle last strip costs almost nothing, while packing it
   // across planes (AfbCfg<L, PW<32>, kept for reference) needs a second launch that costs more than it saves.
   const int n_strips = (p.Wo + 63) / 64;
-  return launch_afb_part<L, 32>(p, stream, n_strips, 0);
+  return launch_afb_part<L, 32, PK>(p, stream, n_strips, 0);
 }
 
-int try_launch_afb(const AfbParams& p, cudaStream_t stream) {
+template <bool PK>
+inline int try_launch_afb_layout(const AfbParams& p, cudaStream_t stream) {
   if (p.Lw != p.Lh) return kNoFastPath;
   if (p.planes == 0) return 0;
   switch (p.Lw) {
-    case 2: return launch_afb_stream<2>(p, stream);
-    case 4: return launch_afb_stream<4>(p, stream);
-    case 6: return launch_afb_stream<6>(p, stream);
-    case 8: return launch_afb_stream<8>(p, stream);
-    case 10: return launch_afb_stream<10>(p, stream);
-    case 12: return launch_afb_stream<12>(p, stream);
-    case 14: return launch_afb_stream<14>(p, stream);
-    case 16: return launch_afb_stream<16>(p, stream);
-    case 18: return launch_afb_stream<18>(p, stream);
-    case 20: return launch_afb_stream<20>(p, stream);
+    case 2: return launch_afb_stream<2, PK>(p, stream);
+    case 4: return launch_afb_stream<4, PK>(p, stream);
+    case 6: return launch_afb_stream<6, PK>(p, stream);
+    case 8: return launch_afb_stream<8, PK>(p, stream);
+    case 10: return launch_afb_stream<10, PK>(p, stream);
+    case 12: return launch_afb_stream<12, PK>(p, stream);
+    case 14: return launch_afb_stream<14, PK>(p, stream);
+    case 16: return launch_afb_stream<16, PK>(p, stream);
+    case 18: return launch_afb_stream<18, PK>(p, stream);
+    case 20: return launch_afb_stream<20, PK>(p, stream);
     default: return kNoFastPath;
   }
 }
+
 
 }  // namespace fast
 }  // namespace b200w

@@ -118,7 +118,7 @@ struct AfbParamsT {  // K1
   int planes, H, W, Ho, Wo, Lw, Lh, mode;
   int tiles_x, tiles_y;
   TapsT<T> fw_lo, fw_hi, fh_lo, fh_hi;
-  int hipitch;        // experiments only (streaming kernel): row pitch of the band-pass planes, 0 = Wo
+  int hipitch;        // row pitch of the band-pass planes (the packet layout, wpt2d.cu), 0 = Wo
   // the W-pass taps once more as interleaved {low-pass, high-pass} pairs: one aligned 64-bit constant load feeds a
   // packed FMA (pairs built from two separate arrays cost two extra uniform moves per FMA pair)
   alignas(16) T fwp[2 * kMaxTaps];

@@ -16,6 +16,9 @@ constexpr int kNoFastPath = 1;
 
 int try_launch_afb(const AfbParams& p, cudaStream_t stream);
 int try_launch_sfb(const SfbParams& p, cudaStream_t stream);
+// the same levels on the wavelet-packet layout (children 4p .. 4p+3 of plane p; see wpt2d.cu)
+int try_launch_wpt_afb(const AfbParams& p, cudaStream_t stream);
+int try_launch_wpt_sfb(const SfbParams& p, cudaStream_t stream);
 int try_launch_fwd_j1(const DtParams& p, cudaStream_t stream);
 int try_launch_scat_j1(const DtParams& p, cudaStream_t stream);
 int try_launch_fwd_j2plus(const DtParams& p, cudaStream_t stream);

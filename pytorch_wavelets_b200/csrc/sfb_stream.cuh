@@ -141,114 +141,16 @@ __device__ __forceinline__ void sfb_stage_dispatch(int vv, const SfbParams& p, c
   }
 }
 
-template <int L, bool PER = false>
-__global__ void __launch_bounds__(32) sfb2d_stream(const __grid_constant__ SfbParams p, int n_strips, int n_chunks,
-                                                   int CH /* output row pairs per chunk */) {
-  using C = SfbCfg<L>;
-  extern __shared__ __align__(16) float ring[];
-  const int lane = threadIdx.x;
-  long long item = blockIdx.x;
-  const int strip = (int)(item % n_strips);
-  item /= n_strips;
-  const int chunk = (int)(item % n_chunks);
-  const int plane = (int)(item / n_chunks);
-
-  const int c0 = strip * 64;                       // first coefficient column (= pair index) of the strip
-  const int npairs_h = PER ? p.Hc : (p.Ho + 1) >> 1;
-  const int m0 = chunk * CH;
-  const int m1 = imin(m0 + CH, npairs_h);
-  const int n_rows = (m1 - m0) + C::HALF - 1;      // coefficient rows m0 .. m1-1+HALF-1
-  const int n_stage = (n_rows + C::KR - 1) / C::KR;
-
-  // zero the ring once: positions that are never copied (columns beyond Wc, absent band-passes) must read 0
-  for (int i = lane; i < C::NS * C::STAGE; i += 32) ring[i] = 0.f;
-  __syncwarp();
-
-  const long long band = (long long)p.Hc * p.Wc;
-  const float* bptr[4];
-  int bpitch[4];
-  bptr[0] = p.ll + (long long)plane * p.llps;
-  bpitch[0] = p.llpitch;
-#pragma unroll
-  for (int b = 1; b < 4; ++b) {
-    bptr[b] = p.highs ? p.highs + ((long long)plane * 3 + (b - 1)) * band : nullptr;
-    bpitch[b] = p.Wc;
-  }
-  // the three 32-lane column copies of a band row: coefficient columns c0 + lane + {0, 32, 64}; PER wraps them
-  int colw[3];
-  bool okc[3];
-#pragma unroll
-  for (int j = 0; j < 3; ++j) {
-    const int cidx = c0 + lane + 32 * j;
-    const bool in_lanes = (j < 2) || (lane < C::HALF - 1);
-    okc[j] = in_lanes && (PER ? (cidx < p.Wc + C::HALF - 1) : (cidx < p.Wc));
-    colw[j] = PER ? cidx % p.Wc : cidx;
-  }
-
-  const unsigned ring_s = (unsigned)__cvta_generic_to_shared(ring) + 4 * lane;
-  int slot_i = 0;
-  auto issue = [&](int t) {
-    const int slot = slot_i;
-    slot_i = (slot_i + 1 == C::NS) ? 0 : slot_i + 1;
-    if (t < n_stage) {
-      const unsigned dst = ring_s + slot * (C::STAGE * 4);
-#pragma unroll
-      for (int r = 0; r < C::KR; ++r) {
-        int k = m0 + C::KR * t + r;
-        bool row_ok = (C::KR * t + r < n_rows);
-        if (PER) k %= p.Hc; else row_ok = row_ok && (k < p.Hc);
-        if (row_ok) {
-#pragma unroll
-          for (int b = 0; b < 4; ++b) {
-            if (bptr[b] == nullptr) continue;
-            const float* src = bptr[b] + (long long)k * bpitch[b];
-            const unsigned d = dst + (r * 4 + b) * (C::SWB * 4);
-            if (okc[0]) cp_async4_s(d, src + colw[0]);
-            if (okc[1]) cp_async4_s(d + 128, src + colw[1]);
-            if (okc[2]) cp_async4_s(d + 256, src + colw[2]);
-          }
-        }
-      }
-    }
-    cp_async_commit();
-  };
-#pragma unroll 1
-  for (int t = 0; t < C::NS - 1; ++t) issue(t);
-
-  float2 wP[C::HALF][2], wQ[C::HALF][2];
-#pragma unroll
-  for (int j = 0; j < C::HALF; ++j)
-#pragma unroll
-    for (int c = 0; c < 2; ++c) { wP[j][c] = make_float2(0.f, 0.f); wQ[j][c] = make_float2(0.f, 0.f); }
-
-  const int col0 = 2 * c0 + 4 * lane;
-  float* y_ptr = PER ? p.y + (long long)plane * p.yps
-                     : p.y + (long long)plane * p.yps + (long long)(2 * m0) * p.ypitch + col0;
-  const int nv4 = imax(0, imin(4, p.Wo - col0));
-  int ncol[4] = {-1, -1, -1, -1};
-  if (PER) {
-    const int N = 2 * p.Wc;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int c = (col0 + q + C::HALF - 1) % N;
-      ncol[q] = (col0 + q < N && c < p.Wo) ? c : -1;
-    }
-  }
-
-  int vv = 0, slot_a = 0;
-#pragma unroll 1
-  for (int t = 0; t < n_stage; ++t) {
-    cp_async_wait<C::NS - 2>();
-    __syncwarp();
-    issue(t + C::NS - 1);
-    const float* stage = ring + slot_a * C::STAGE + 2 * lane;
-    slot_a = (slot_a + 1 == C::NS) ? 0 : slot_a + 1;
-    sfb_stage_dispatch<L, 0, PER>(vv, p, stage, wP, wQ, C::KR * t, n_rows, m0, y_ptr, p.ypitch, nv4, ncol);
-    vv = (vv + 1 == C::UNS) ? 0 : vv + 1;
-  }
-  cp_async_wait<0>();
-}
-
+#define B200W_SFB_KERNEL sfb2d_stream
+#define B200W_SFB_PLANE_BANDS 3
+#include "sfb_stream_kernel.cuh"
+#undef B200W_SFB_KERNEL
+#undef B200W_SFB_PLANE_BANDS
+#define B200W_SFB_KERNEL wpt_sfb2d_stream
+#define B200W_SFB_PLANE_BANDS 4
+#include "sfb_stream_kernel.cuh"
+#undef B200W_SFB_KERNEL
+#undef B200W_SFB_PLANE_BANDS
 
 // ------------------------------------------------------------------------------------------------------------------
 // Wide form (filters up to 8 taps, every mode except periodization): a lane owns FOUR coefficient columns (eight
@@ -359,159 +261,95 @@ __device__ __forceinline__ void sfb4_stage_dispatch(int vv, const SfbParams& p, 
   }
 }
 
-template <int L>
-__global__ void __launch_bounds__(32) sfb2d_stream4(const __grid_constant__ SfbParams p, int n_strips, int n_chunks,
-                                                    int CH /* output row pairs per chunk */) {
-  using C = Sfb4Cfg<L>;
-  extern __shared__ __align__(16) float ring[];
-  const int lane = threadIdx.x;
-  long long item = blockIdx.x;
-  const int strip = (int)(item % n_strips);
-  item /= n_strips;
-  const int chunk = (int)(item % n_chunks);
-  const int plane = (int)(item / n_chunks);
+#define B200W_SFB4_KERNEL sfb2d_stream4
+#define B200W_SFB_PLANE_BANDS 3
+#include "sfb_stream4_kernel.cuh"
+#undef B200W_SFB4_KERNEL
+#undef B200W_SFB_PLANE_BANDS
+#define B200W_SFB4_KERNEL wpt_sfb2d_stream4
+#define B200W_SFB_PLANE_BANDS 4
+#include "sfb_stream4_kernel.cuh"
+#undef B200W_SFB4_KERNEL
+#undef B200W_SFB_PLANE_BANDS
 
-  const int c0 = strip * C::CW;                    // first coefficient column (= output column pair) of the strip
-  const int npairs_h = (p.Ho + 1) >> 1;
-  const int m0 = chunk * CH;
-  const int m1 = imin(m0 + CH, npairs_h);
-  const int n_rows = (m1 - m0) + C::HALF - 1;      // coefficient rows m0 .. m1-1+HALF-1
-  const int n_stage = (n_rows + C::KR - 1) / C::KR;
-
-  // zero the ring once: positions that are never copied (columns beyond Wc, absent band-passes) must read 0
-  for (int i = lane; i < C::NS * C::STAGE; i += 32) ring[i] = 0.f;
-  __syncwarp();
-
-  const long long band = (long long)p.Hc * p.Wc;
-  const float* bptr[4];
-  int bpitch[4];
-  bptr[0] = p.ll + (long long)plane * p.llps;
-  bpitch[0] = p.llpitch;
-#pragma unroll
-  for (int b = 1; b < 4; ++b) {
-    bptr[b] = p.highs ? p.highs + ((long long)plane * 3 + (b - 1)) * band : nullptr;
-    bpitch[b] = p.Wc;
+// the DWT-layout or the packet-layout kernel (only the one asked for is instantiated)
+template <int L, bool PER, bool PK, bool WIDE>
+constexpr auto sfb_kernel_of() {
+  if constexpr (WIDE) {
+    if constexpr (PK) return wpt_sfb2d_stream4<L>;
+    else return sfb2d_stream4<L>;
+  } else {
+    if constexpr (PK) return wpt_sfb2d_stream<L, PER>;
+    else return sfb2d_stream<L, PER>;
   }
-  // the 32-lane column copies of a band row: coefficient columns c0 + lane + 32 j
-  unsigned okmask = 0;
-#pragma unroll
-  for (int j = 0; j < C::NCOPY; ++j)
-    if ((lane + 32 * j < C::CW + C::HALF - 1) && (c0 + lane + 32 * j < p.Wc)) okmask |= 1u << j;
-
-  const unsigned ring_s = (unsigned)__cvta_generic_to_shared(ring) + 4 * lane;
-  int slot_i = 0;
-  auto issue = [&](int t) {
-    const int slot = slot_i;
-    slot_i = (slot_i + 1 == C::NS) ? 0 : slot_i + 1;
-    if (t < n_stage) {
-      const unsigned dst = ring_s + slot * (C::STAGE * 4);
-#pragma unroll
-      for (int r = 0; r < C::KR; ++r) {
-        const int k = m0 + C::KR * t + r;
-        if ((C::KR * t + r < n_rows) && (k < p.Hc)) {
-#pragma unroll
-          for (int b = 0; b < 4; ++b) {
-            if (bptr[b] == nullptr) continue;
-            const float* src = bptr[b] + (long long)k * bpitch[b] + c0 + lane;
-            const unsigned d = dst + (r * 4 + b) * (C::SWB * 4);
-#pragma unroll
-            for (int j = 0; j < C::NCOPY; ++j)
-              if (okmask & (1u << j)) cp_async4_s(d + 128 * j, src + 32 * j);
-          }
-        }
-      }
-    }
-    cp_async_commit();
-  };
-#pragma unroll 1
-  for (int t = 0; t < C::NS - 1; ++t) issue(t);
-
-  float2 wP[C::HALF][4], wQ[C::HALF][4];
-#pragma unroll
-  for (int j = 0; j < C::HALF; ++j)
-#pragma unroll
-    for (int c = 0; c < 4; ++c) { wP[j][c] = make_float2(0.f, 0.f); wQ[j][c] = make_float2(0.f, 0.f); }
-
-  const int col0 = 2 * c0 + 8 * lane;
-  float* y_ptr = p.y + (long long)plane * p.yps + (long long)(2 * m0) * p.ypitch + col0;
-  const int nv8 = imax(0, imin(8, p.Wo - col0));
-
-  int vv = 0, slot_a = 0;
-#pragma unroll 1
-  for (int t = 0; t < n_stage; ++t) {
-    cp_async_wait<C::NS - 2>();
-    __syncwarp();
-    issue(t + C::NS - 1);
-    const float* stage = ring + slot_a * C::STAGE + 4 * lane;
-    slot_a = (slot_a + 1 == C::NS) ? 0 : slot_a + 1;
-    sfb4_stage_dispatch<L, 0>(vv, p, stage, wP, wQ, C::KR * t, n_rows, m0, y_ptr, p.ypitch, nv8);
-    vv = (vv + 1 == C::UNS) ? 0 : vv + 1;
-  }
-  cp_async_wait<0>();
 }
 
-template <int L>
+template <int L, bool PK>
 inline int launch_sfb_stream4(const SfbParams& p, cudaStream_t stream, int n_strips) {
   using C = Sfb4Cfg<L>;
+  constexpr auto kernel = sfb_kernel_of<L, false, PK, true>();
   const int npairs_h = (p.Ho + 1) >> 1;
   int n_chunks, CH;
   static ConcCache conc_cache;
-  const int conc = resident_warps_dev(conc_cache, sfb2d_stream4<L>, C::SMEM_BYTES);
+  const int conc = resident_warps_dev(conc_cache, kernel, C::SMEM_BYTES);
   pick_chunks((long long)p.planes * n_strips, npairs_h, 16, L / 2 + 8, conc, &n_chunks, &CH);
   const long long blocks = (long long)p.planes * n_strips * n_chunks;
   if (blocks <= 0) return 0;
   if (blocks > 2147483647LL) return kNoFastPath;
-  sfb2d_stream4<L><<<(unsigned)blocks, 32, C::SMEM_BYTES, stream>>>(p, n_strips, n_chunks, CH);
+  kernel<<<(unsigned)blocks, 32, C::SMEM_BYTES, stream>>>(p, n_strips, n_chunks, CH);
   return 0;
 }
 
-template <int L, bool PER>
+template <int L, bool PER, bool PK>
 inline int launch_sfb_stream_m(const SfbParams& p, cudaStream_t stream) {
   using C = SfbCfg<L>;
+  constexpr auto kernel = sfb_kernel_of<L, PER, PK, false>();
   const int npairs_w = PER ? p.Wc : (p.Wo + 1) >> 1;
   const int npairs_h = PER ? p.Hc : (p.Ho + 1) >> 1;
   const int n_strips = (npairs_w + 63) / 64;
   int n_chunks, CH;
   static ConcCache conc_cache;
-  const int conc = resident_warps_dev(conc_cache, sfb2d_stream<L, PER>, C::SMEM_BYTES);
+  const int conc = resident_warps_dev(conc_cache, kernel, C::SMEM_BYTES);
   pick_chunks((long long)p.planes * n_strips, npairs_h, 16, L / 2 + 8, conc, &n_chunks, &CH);
   const long long blocks = (long long)p.planes * n_strips * n_chunks;
   if (blocks <= 0) return 0;
   if (blocks > 2147483647LL) return kNoFastPath;
-  sfb2d_stream<L, PER><<<(unsigned)blocks, 32, C::SMEM_BYTES, stream>>>(p, n_strips, n_chunks, CH);
+  kernel<<<(unsigned)blocks, 32, C::SMEM_BYTES, stream>>>(p, n_strips, n_chunks, CH);
   return 0;
 }
 
-template <int L>
+template <int L, bool PK>
 inline int launch_sfb_stream(const SfbParams& p, cudaStream_t stream) {
-  if (p.mode == B200W_MODE_PERIODIZATION) return launch_sfb_stream_m<L, true>(p, stream);
+  if (p.mode == B200W_MODE_PERIODIZATION) return launch_sfb_stream_m<L, true, PK>(p, stream);
   if constexpr (L <= 8) {
     // 128-column strips for every plane with more than 64 column pairs, remainder strip included: routing a narrow
     // remainder to the 2-column kernel in a second launch costs more than it saves, and one 67-pair wide strip beats a
     // 64 + 3 pair of narrow ones
     const int npairs_w = (p.Wo + 1) >> 1;
-    if (npairs_w > 64) return launch_sfb_stream4<L>(p, stream, (npairs_w + 127) / 128);
+    if (npairs_w > 64) return launch_sfb_stream4<L, PK>(p, stream, (npairs_w + 127) / 128);
   }
-  return launch_sfb_stream_m<L, false>(p, stream);
+  return launch_sfb_stream_m<L, false, PK>(p, stream);
 }
 
-int try_launch_sfb(const SfbParams& p, cudaStream_t stream) {
+template <bool PK>
+inline int try_launch_sfb_layout(const SfbParams& p, cudaStream_t stream) {
   if (p.Lw != p.Lh) return kNoFastPath;
   if (p.planes == 0) return 0;
   switch (p.Lw) {
-    case 2: return launch_sfb_stream<2>(p, stream);
-    case 4: return launch_sfb_stream<4>(p, stream);
-    case 6: return launch_sfb_stream<6>(p, stream);
-    case 8: return launch_sfb_stream<8>(p, stream);
-    case 10: return launch_sfb_stream<10>(p, stream);
-    case 12: return launch_sfb_stream<12>(p, stream);
-    case 14: return launch_sfb_stream<14>(p, stream);
-    case 16: return launch_sfb_stream<16>(p, stream);
-    case 18: return launch_sfb_stream<18>(p, stream);
-    case 20: return launch_sfb_stream<20>(p, stream);
+    case 2: return launch_sfb_stream<2, PK>(p, stream);
+    case 4: return launch_sfb_stream<4, PK>(p, stream);
+    case 6: return launch_sfb_stream<6, PK>(p, stream);
+    case 8: return launch_sfb_stream<8, PK>(p, stream);
+    case 10: return launch_sfb_stream<10, PK>(p, stream);
+    case 12: return launch_sfb_stream<12, PK>(p, stream);
+    case 14: return launch_sfb_stream<14, PK>(p, stream);
+    case 16: return launch_sfb_stream<16, PK>(p, stream);
+    case 18: return launch_sfb_stream<18, PK>(p, stream);
+    case 20: return launch_sfb_stream<20, PK>(p, stream);
     default: return kNoFastPath;
   }
 }
+
 
 
 }  // namespace fast

@@ -31,7 +31,9 @@ B200W_HD int afb_smem_floats(int Lw, int Lh) {
   return IH * IWp + 2 * IH * kAfbTW;
 }
 
-template <int NT, class T>
+// PK (packet layout): child b of plane p goes to ll + (4p + b) * (llps / 4) with row pitch llpitch; `highs` is then
+// ll + llps / 4 and `hipitch` the row pitch of the band-pass children.
+template <int NT, class T, bool PK = false>
 B200W_D void afb2d_tile(const AfbParamsT<T>& p, int bid, T* smem) {
   constexpr int TH = kAfbTH, TW = kAfbTW;
   const int tx = bid % p.tiles_x;
@@ -94,8 +96,15 @@ B200W_D void afb2d_tile(const AfbParamsT<T>& p, int bid, T* smem) {
         ahh = fma_rn(f1, vhi, ahh);
       }
       p.ll[(long long)plane * p.llps + (long long)orow * p.llpitch + ocol] = all;
-      const long long band = (long long)p.Ho * p.Wo;
-      T* hp = p.highs + (long long)plane * 3 * band + (long long)orow * p.Wo + ocol;
+      long long band;
+      T* hp;
+      if constexpr (PK) {
+        band = p.llps >> 2;
+        hp = p.highs + (long long)plane * p.llps + (long long)orow * p.hipitch + ocol;
+      } else {
+        band = (long long)p.Ho * p.Wo;
+        hp = p.highs + (long long)plane * 3 * band + (long long)orow * p.Wo + ocol;
+      }
       hp[0] = alh;
       hp[band] = ahl;
       hp[2 * band] = ahh;
@@ -116,7 +125,9 @@ B200W_HD int sfb_smem_floats(int Lh, int Lw) {
   return 4 * KH * KW + 2 * kSfbTH * KW;
 }
 
-template <int NT, class T>
+// PK (packet layout): the four children of plane p are planes 4p .. 4p+3 of one contiguous (4P, Hc, Wc) tensor: `ll`
+// = its base with llps = 4 Hc Wc, `highs` = ll + Hc Wc.
+template <int NT, class T, bool PK = false>
 B200W_D void sfb2d_tile(const SfbParamsT<T>& p, int bid, T* smem) {
   constexpr int TH = kSfbTH, TW = kSfbTW;
   const int tx = bid % p.tiles_x;
@@ -140,7 +151,7 @@ B200W_D void sfb2d_tile(const SfbParamsT<T>& p, int bid, T* smem) {
   T* s_hi = s_lo + TH * KW;
   const T* llp = p.ll + (long long)plane * p.llps;
   const long long band = (long long)p.Hc * p.Wc;
-  const T* hp = p.highs ? p.highs + (long long)plane * 3 * band : nullptr;
+  const T* hp = p.highs ? p.highs + (long long)plane * (PK ? 4 : 3) * band : nullptr;
 
   B200W_FOR_THREADS(tid, NT)
     for (int idx = tid; idx < KH * KW; idx += NT) {
