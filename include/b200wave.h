@@ -142,6 +142,38 @@ int b200w_dwt_sfb1d(const float* lo, const float* hi, int rows, int K, float* y,
                     const float* g0, const float* g1, int L, int mode, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Transpose of the mode-extended analysis bank (an addition beyond the reference): the exact adjoint A_m^T of
+ * b200w_dwt_afb2d / b200w_dwt_afb1d in every mode, which SFB2D / SFB1D's double backward needs (the reference gets it
+ * by differentiating its backward's F.pad / conv2d graph, dwt/lowlevel.py:683-694, 732-743).  It differs from the
+ * synthesis bank (K2 cropped to n) in symmetric, reflect, periodic and odd-size periodization mode, where the boundary
+ * extension folds the coefficients that reach extended positions back onto the samples they copy.
+ *   b200w_dwt_afb2d_adjoint: ll (planes, Hc, Wc) pitched, highs (planes, 3, Hc, Wc) contiguous or NULL = zeros
+ *                            -> y (planes, H, W) pitched, with Hc = b200w_dwt_coeff_len(H, Lh, mode) and
+ *                            Wc = b200w_dwt_coeff_len(W, Lw, mode).  fh_*: the stored analysis taps of the H pass,
+ *                            fw_* of the W pass (b200w_dwt_afb2d's fh / fw).
+ *   b200w_dwt_afb1d_adjoint: lo, hi (rows, K) contiguous (hi may be NULL) -> y (rows, N) contiguous,
+ *                            K = b200w_dwt_coeff_len(N, L, mode).
+ * One call is the synthesis level cropped to the output (the streaming kernels where they apply) followed, outside zero
+ * mode and even-size periodization, by one border kernel that rewrites the outputs within L samples of an edge.
+ * Errors: B200W_EMODE, B200W_EARG for a NULL required pointer or a pitch below the row length, B200W_ESIZE for a
+ * coefficient size that is not the analysis length of the output size, B200W_EFILTER for L < 2 or L > 40.
+ */
+int b200w_dwt_afb2d_adjoint(const float* ll, long long ll_plane_stride, int ll_pitch, const float* highs,
+                            float* y, long long y_plane_stride, int y_pitch,
+                            int planes, int Hc, int Wc, int H, int W,
+                            const float* fh_lo, const float* fh_hi, int Lh,
+                            const float* fw_lo, const float* fw_hi, int Lw, int mode, void* stream);
+int b200w_dwt_afb2d_adjoint_f64(const double* ll, long long ll_plane_stride, int ll_pitch, const double* highs,
+                                double* y, long long y_plane_stride, int y_pitch,
+                                int planes, int Hc, int Wc, int H, int W,
+                                const double* fh_lo, const double* fh_hi, int Lh,
+                                const double* fw_lo, const double* fw_hi, int Lw, int mode, void* stream);
+int b200w_dwt_afb1d_adjoint(const float* lo, const float* hi, int rows, int K, float* y, int N,
+                            const float* f0, const float* f1, int L, int mode, void* stream);
+int b200w_dwt_afb1d_adjoint_f64(const double* lo, const double* hi, int rows, int K, double* y, int N,
+                                const double* f0, const double* f1, int L, int mode, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * 3-D DWT levels (an addition beyond the reference; DWT3DForward / DWT3DInverse).  One filter pair acts along all
  * three axes.  Analysis = the 1-D analysis along W, then H, then D, each pass rounded to the element type; synthesis is
  * the reverse (along D, then the 2-D synthesis: H, then W).  Per axis the sizes follow b200w_dwt_coeff_len /

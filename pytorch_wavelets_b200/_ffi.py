@@ -38,7 +38,8 @@ SYMBOLS = SYMBOLS + [s + '_generic' for s in KERNEL_ENTRIES] + [s + '_f64' for s
     'b200w_dtcwt1d_%s%s' % (k, v) for k in ('fwd_j1', 'fwd_j2plus', 'inv_j1', 'inv_j2plus') for v in ('', '_f64')] + [
     'b200w_dtcwt_fwd_j12', 'b200w_dtcwt_fwd_j12_generic', 'b200w_dtcwt_fwd_j12_workspace'] + [
     'b200w_scat1d_%s%s' % (k, v) for k in ('j1', 'j2plus') for v in ('', '_f64')] + [
-    'b200w_wpt_%s2d%s' % (k, v) for k in ('afb', 'sfb') for v in ('', '_generic', '_f64')]
+    'b200w_wpt_%s2d%s' % (k, v) for k in ('afb', 'sfb') for v in ('', '_generic', '_f64')] + [
+    'b200w_dwt_afb%dd_adjoint%s' % (d, v) for d in (2, 1) for v in ('', '_f64')]
 
 
 class B200WaveError(RuntimeError):
@@ -122,6 +123,12 @@ def lib():
                                                           pf, pf, c_int, pf, pf, c_int, c_int, c_vp]
             getattr(L, 'b200w_wpt_sfb2d' + v).argtypes = [c_vp, c_vp, c_ll, c_int, c_int, c_int, c_int, c_int, c_int,
                                                           pf, pf, c_int, pf, pf, c_int, c_int, c_vp]
+        for v in ('', '_f64'):   # transpose of the analysis bank (csrc/dwt_adjoint.cu)
+            getattr(L, 'b200w_dwt_afb2d_adjoint' + v).argtypes = [c_vp, c_ll, c_int, c_vp, c_vp, c_ll, c_int, c_int,
+                                                                  c_int, c_int, c_int, c_int, pf, pf, c_int, pf, pf,
+                                                                  c_int, c_int, c_vp]
+            getattr(L, 'b200w_dwt_afb1d_adjoint' + v).argtypes = [c_vp, c_vp, c_int, c_int, c_vp, c_int, pf, pf, c_int,
+                                                                  c_int, c_vp]
         L.b200w_dtcwt_fwd_j12_workspace.argtypes = [c_vp, c_ll, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
                                                     c_int]
         L.b200w_dtcwt_fwd_j12_workspace.restype = c_ll

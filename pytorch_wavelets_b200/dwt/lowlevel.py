@@ -157,6 +157,50 @@ def sfb2d_level(ll, highs, gh_lo, gh_hi, gw_lo, gw_hi, mode, out_hw=None):
     return y
 
 
+def afb2d_adjoint_level(ll, highs, fh_lo, fh_hi, fw_lo, fw_hi, mode, out_hw):
+    """The transpose of ``afb2d_level`` in mode ``mode`` (``b200w_dwt_afb2d_adjoint``): ll (N,C,Hc,Wc) and highs
+    (N,C,3,Hc,Wc) -> (N,C,H,W) with ``(H, W) = out_hw``, the analysis input size.  ``fh_*`` / ``fw_*``: the stored
+    analysis taps along H / W.  Equals ``sfb2d_level(..., out_hw=out_hw)`` in zero mode and even-size
+    periodization (the C entry then launches only the synthesis kernel); elsewhere the boundary extension is folded
+    back onto the samples it copies."""
+    dt = _ffi.require_cuda_real(ll, 'low')
+    _check_bank_mode(mode)
+    L = _ffi.lib()
+    fh_lo, fh_hi = _taps_pair(fh_lo, fh_hi)
+    fw_lo, fw_hi = _taps_pair(fw_lo, fw_hi)
+    N, C, Hc, Wc = ll.shape
+    H, W = int(out_hw[0]), int(out_hw[1])
+    if Hc != L.b200w_dwt_coeff_len(H, fh_lo.n, mode) or Wc != L.b200w_dwt_coeff_len(W, fw_lo.n, mode):
+        raise ValueError('coefficients {}x{} are not the analysis of a {}x{} input'.format(Hc, Wc, H, W))
+    if highs is not None:
+        _ffi.require_cuda_real(highs, 'highs', dt)
+        if tuple(highs.shape) != (N, C, 3, Hc, Wc):
+            raise ValueError('highs shape {} does not match low shape {}'.format(tuple(highs.shape), tuple(ll.shape)))
+        highs = highs.contiguous()
+    ll, llps, llpitch = _ffi.planes_view(ll)
+    y = ll.new_empty((N, C, H, W))
+    if N * C > 0:
+        with torch.cuda.device(ll.device), _ffi.span('dwt_afb2d_adjoint %dx%d L%d' % (Hc, Wc, fh_lo.n),
+                                                     ll.element_size() * N * C * ((1 if highs is None else 4) * Hc * Wc + H * W)):
+            rc = _ffi.entry('b200w_dwt_afb2d_adjoint', dt)(
+                ll.data_ptr(), llps, llpitch, None if highs is None else highs.data_ptr(), y.data_ptr(), H * W, W,
+                N * C, Hc, Wc, H, W, fh_lo.p(dt), fh_hi.p(dt), fh_lo.n, fw_lo.p(dt), fw_hi.p(dt), fw_lo.n, mode,
+                _ffi.stream_of(ll))
+        _ffi.check(rc, 'b200w_dwt_afb2d_adjoint')
+    return y
+
+
+def _pad_odd(x, dims):
+    """x with one zero appended along each dimension of ``dims`` whose size is odd (the periodization analysis of an
+    odd-size signal is the analysis of the signal padded to even size)."""
+    for d in dims:
+        if x.shape[d] % 2:
+            shape = list(x.shape)
+            shape[d] = 1
+            x = torch.cat([x, x.new_zeros(shape)], dim=d)
+    return x
+
+
 def dwt_forward_levels(x, fw_lo, fw_hi, fh_lo, fh_hi, mode, J):
     """All J analysis levels through ONE C-ABI call (``b200w_dwt_forward``): a single fused kernel launch when the
     pyramid kernel applies (no inter-level low-pass in device memory), one launch per level otherwise.
@@ -289,7 +333,7 @@ class AFB2D(Function):
     ``forward(ctx, x, h0_row, h1_row, h0_col, h1_col, mode)``: the ``*_row`` filters act along W
     (dim 3) and the ``*_col`` filters along H (dim 2), exactly as in the reference (:341-342).
     Returns ``(low (N,C,H',W'), highs (N,C,3,H',W'))``.  The backward pass is the synthesis kernel
-    with the same stored filters, cropped to the input size (:350-365).
+    with the same stored filters, cropped to the input size (:350-365), as the differentiable ``SynthesisCrop2D``.
     """
 
     @staticmethod
@@ -307,7 +351,7 @@ class AFB2D(Function):
         dx = None
         if ctx.needs_input_grad[0]:
             h0_row, h1_row, h0_col, h1_col = ctx.taps
-            dx = sfb2d_level(low, highs, h0_col, h1_col, h0_row, h1_row, ctx.mode, out_hw=ctx.shape)
+            dx = SynthesisCrop2D.apply(low, highs, h0_col, h1_col, h0_row, h1_row, ctx.mode, ctx.shape)
         return dx, None, None, None, None, None, None
 
 
@@ -315,7 +359,8 @@ class SFB2D(Function):
     """Single-level 2-D synthesis filter bank; drop-in for the reference ``SFB2D`` (dwt/lowlevel.py:647-694).
 
     ``forward(ctx, low, highs, g0_row, g1_row, g0_col, g1_col, mode)``: ``*_col`` filters act along H
-    first (:677-678), then ``*_row`` along W (:679).  ``highs`` may be None (treated as zeros).
+    first (:677-678), then ``*_row`` along W (:679).  ``highs`` may be None (treated as zeros).  The backward pass
+    is the analysis with the same filters in the same mode (:683-694), as the differentiable ``Analysis2D``.
     """
 
     @staticmethod
@@ -333,7 +378,7 @@ class SFB2D(Function):
         dlow, dhigh = None, None
         if ctx.needs_input_grad[0] or (ctx.has_highs and ctx.needs_input_grad[1]):
             g0_row, g1_row, g0_col, g1_col = ctx.taps
-            dlow, dhigh = afb2d_level(dy.contiguous(), g0_row, g1_row, g0_col, g1_col, ctx.mode)
+            dlow, dhigh = Analysis2D.apply(dy.contiguous(), g0_col, g1_col, g0_row, g1_row, ctx.mode)
             if not ctx.has_highs:
                 dhigh = None
         return dlow, dhigh, None, None, None, None, None
@@ -344,7 +389,7 @@ class DWTPyramid(Function):
     ``apply(x, h0_row, h1_row, h0_col, h1_col, mode, J) -> (yl, yh_1, ..., yh_J)`` with the filter arguments of
     ``AFB2D`` (``*_row`` along W, ``*_col`` along H).  Forward = one fused kernel launch where the pyramid kernel
     applies; backward = the reference's chain of ``AFB2D.backward`` (synthesis with the stored analysis filters,
-    cropped to each level's input size, dwt/lowlevel.py:350-365)."""
+    cropped to each level's input size, dwt/lowlevel.py:350-365), one ``SynthesisCrop2D`` per level."""
 
     @staticmethod
     def forward(ctx, x, h0_row, h1_row, h0_col, h1_col, mode, J):
@@ -366,9 +411,95 @@ class DWTPyramid(Function):
                 sh = ctx.in_shapes[j]
                 if low is None:
                     low = dyh[j].new_zeros(dyh[j].shape[:2] + dyh[j].shape[-2:])
-                low = sfb2d_level(low.contiguous(), dyh[j], h0_col, h1_col, h0_row, h1_row, ctx.mode, out_hw=sh)
+                low = SynthesisCrop2D.apply(low.contiguous(), dyh[j], h0_col, h1_col, h0_row, h1_row, ctx.mode, sh)
             dx = low
         return dx, None, None, None, None, None, None
+
+
+# ---- the backward passes as autograd Functions (double backward) ------------------------------------------
+# Each first-order backward above is one of the four operators below, and each operator's backward is its exact
+# transpose, which is again one of them.  So a graph built with create_graph=True differentiates to any order, as the
+# reference's torch-op backward passes do.  With grad mode off (a plain .backward()) ``apply`` runs only the forward:
+# the same kernel call, with the same arguments, as before these Functions existed.
+#   SynthesisCrop2D   crop_(H,W) . S       <->  SynthesisCrop2DT  S^T . pad = zero-mode analysis (periodization: on the
+#                                                                 input zero-padded to even size)
+#   Analysis2D        A_m                  <->  Analysis2DT       A_m^T (b200w_dwt_afb2d_adjoint)
+# Taps are HostTaps in the synthesis argument order: fh_* along H, fw_* along W.  They stay constants.
+
+class SynthesisCrop2D(Function):
+    """``apply(low, highs, fh_lo, fh_hi, fw_lo, fw_hi, mode, out_hw)``: the synthesis level cropped to ``out_hw``
+    (``AFB2D``'s backward pass).  Its backward pass is ``SynthesisCrop2DT``."""
+
+    @staticmethod
+    def forward(ctx, low, highs, fh_lo, fh_hi, fw_lo, fw_hi, mode, out_hw):
+        ctx.taps, ctx.mode, ctx.out_hw = (fh_lo, fh_hi, fw_lo, fw_hi), mode, tuple(out_hw)
+        ctx.has_highs = highs is not None
+        return sfb2d_level(low, highs, fh_lo, fh_hi, fw_lo, fw_hi, mode, out_hw=out_hw)
+
+    @staticmethod
+    def backward(ctx, dy):
+        dlow = dhigh = None
+        if ctx.needs_input_grad[0] or (ctx.has_highs and ctx.needs_input_grad[1]):
+            dlow, dhigh = SynthesisCrop2DT.apply(dy, *ctx.taps, ctx.mode)
+            if not ctx.has_highs:
+                dhigh = None
+        return dlow, dhigh, None, None, None, None, None, None
+
+
+class SynthesisCrop2DT(Function):
+    """``apply(y, fh_lo, fh_hi, fw_lo, fw_hi, mode) -> (low, highs)``: the transpose of ``SynthesisCrop2D`` for an
+    (H, W) input.  The cropped synthesis does not depend on the mode outside periodization, so this is the zero-mode
+    analysis there; in periodization it is the periodization analysis of y zero-padded to even size."""
+
+    @staticmethod
+    def forward(ctx, y, fh_lo, fh_hi, fw_lo, fw_hi, mode):
+        ctx.taps, ctx.mode, ctx.shape = (fh_lo, fh_hi, fw_lo, fw_hi), mode, tuple(y.shape[-2:])
+        if mode == _MODES['periodization']:
+            y = _pad_odd(y, (-2, -1))
+        else:
+            mode = _MODES['zero']
+        return afb2d_level(y.contiguous(), fw_lo, fw_hi, fh_lo, fh_hi, mode)
+
+    @staticmethod
+    def backward(ctx, dlow, dhighs):
+        dy = None
+        if ctx.needs_input_grad[0]:
+            dy = SynthesisCrop2D.apply(dlow, dhighs, *ctx.taps, ctx.mode, ctx.shape)
+        return dy, None, None, None, None, None
+
+
+class Analysis2D(Function):
+    """``apply(x, fh_lo, fh_hi, fw_lo, fw_hi, mode) -> (low, highs)``: the analysis level in mode ``mode``
+    (``SFB2D``'s backward pass).  Its backward pass is ``Analysis2DT``."""
+
+    @staticmethod
+    def forward(ctx, x, fh_lo, fh_hi, fw_lo, fw_hi, mode):
+        ctx.taps, ctx.mode, ctx.shape = (fh_lo, fh_hi, fw_lo, fw_hi), mode, tuple(x.shape[-2:])
+        return afb2d_level(x, fw_lo, fw_hi, fh_lo, fh_hi, mode)
+
+    @staticmethod
+    def backward(ctx, dlow, dhighs):
+        dx = None
+        if ctx.needs_input_grad[0]:
+            dx = Analysis2DT.apply(dlow, dhighs, *ctx.taps, ctx.mode, ctx.shape)
+        return dx, None, None, None, None, None
+
+
+class Analysis2DT(Function):
+    """``apply(low, highs, fh_lo, fh_hi, fw_lo, fw_hi, mode, out_hw) -> y``: the transpose of ``Analysis2D`` for an
+    ``out_hw`` input (``afb2d_adjoint_level``).  Its backward pass is ``Analysis2D``."""
+
+    @staticmethod
+    def forward(ctx, low, highs, fh_lo, fh_hi, fw_lo, fw_hi, mode, out_hw):
+        ctx.taps, ctx.mode = (fh_lo, fh_hi, fw_lo, fw_hi), mode
+        return afb2d_adjoint_level(low, highs, fh_lo, fh_hi, fw_lo, fw_hi, mode, out_hw)
+
+    @staticmethod
+    def backward(ctx, dy):
+        dlow = dhigh = None
+        if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
+            dlow, dhigh = Analysis2D.apply(dy.contiguous(), *ctx.taps, ctx.mode)
+        return dlow, dhigh, None, None, None, None, None, None
 
 
 class AFB3D(Function):

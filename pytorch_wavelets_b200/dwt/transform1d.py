@@ -56,9 +56,113 @@ def sfb1d_level(lo, hi, g0, g1, mode, out_len=None):
     return y
 
 
+def afb1d_adjoint_level(lo, hi, f0, f1, mode, n):
+    """The transpose of ``afb1d_level`` in mode ``mode`` (``b200w_dwt_afb1d_adjoint``): lo, hi (N, C, K) (hi may be
+    None) -> (N, C, n), n the analysis input length; stored analysis taps.  Equals ``sfb1d_level(..., out_len=n)`` in
+    zero mode and even-size periodization (the C entry then launches only the synthesis kernel)."""
+    dt = _ffi.require_cuda_real(lo, 'low')
+    lowlevel._check_bank_mode(mode)
+    L = _ffi.lib()
+    f0, f1 = lowlevel._taps_pair(f0, f1)
+    lo = lo.contiguous()
+    N, C, K = lo.shape
+    n = int(n)
+    if K != L.b200w_dwt_coeff_len(n, f0.n, mode):
+        raise ValueError('{} coefficients are not the analysis of a length-{} signal'.format(K, n))
+    if hi is not None:
+        _ffi.require_cuda_real(hi, 'high', dt)
+        if tuple(hi.shape) != tuple(lo.shape):
+            raise ValueError('high shape {} does not match low shape {}'.format(tuple(hi.shape), tuple(lo.shape)))
+        hi = hi.contiguous()
+    y = lo.new_empty((N, C, n))
+    if N * C > 0:
+        with torch.cuda.device(lo.device), _ffi.span('dwt_afb1d_adjoint %d L%d' % (K, f0.n),
+                                                     lo.element_size() * N * C * (2 * K + n)):
+            rc = _ffi.entry('b200w_dwt_afb1d_adjoint', dt)(lo.data_ptr(), None if hi is None else hi.data_ptr(),
+                                                           N * C, K, y.data_ptr(), n, f0.p(dt), f1.p(dt), f0.n, mode,
+                                                           _ffi.stream_of(lo))
+        _ffi.check(rc, 'b200w_dwt_afb1d_adjoint')
+    return y
+
+
+# The backward passes as autograd Functions, each the other's transpose (see dwt/lowlevel.py, SynthesisCrop2D):
+#   SynthesisCrop1D  crop_n . S  <->  SynthesisCrop1DT  zero-mode analysis (periodization: of the signal padded to even n)
+#   Analysis1D       A_m         <->  Analysis1DT       A_m^T (b200w_dwt_afb1d_adjoint)
+
+class SynthesisCrop1D(Function):
+    """``apply(lo, hi, f0, f1, mode, n)``: the synthesis cropped to n (``AFB1D``'s backward pass)."""
+
+    @staticmethod
+    def forward(ctx, lo, hi, f0, f1, mode, n):
+        ctx.taps, ctx.mode, ctx.has_hi = (f0, f1), mode, hi is not None
+        return sfb1d_level(lo, hi, f0, f1, mode, out_len=n)
+
+    @staticmethod
+    def backward(ctx, dy):
+        dlo = dhi = None
+        if ctx.needs_input_grad[0] or (ctx.has_hi and ctx.needs_input_grad[1]):
+            dlo, dhi = SynthesisCrop1DT.apply(dy, *ctx.taps, ctx.mode)
+            if not ctx.has_hi:
+                dhi = None
+        return dlo, dhi, None, None, None, None
+
+
+class SynthesisCrop1DT(Function):
+    """``apply(y, f0, f1, mode) -> (lo, hi)``: the transpose of ``SynthesisCrop1D`` for a length-n y."""
+
+    @staticmethod
+    def forward(ctx, y, f0, f1, mode):
+        ctx.taps, ctx.mode, ctx.n = (f0, f1), mode, y.shape[-1]
+        if mode == lowlevel._MODES['periodization']:
+            y = lowlevel._pad_odd(y, (-1,))
+        else:
+            mode = lowlevel._MODES['zero']
+        return afb1d_level(y, f0, f1, mode)
+
+    @staticmethod
+    def backward(ctx, dlo, dhi):
+        dy = None
+        if ctx.needs_input_grad[0]:
+            dy = SynthesisCrop1D.apply(dlo, dhi, *ctx.taps, ctx.mode, ctx.n)
+        return dy, None, None, None
+
+
+class Analysis1D(Function):
+    """``apply(x, f0, f1, mode) -> (lo, hi)``: the analysis in mode ``mode`` (``SFB1D``'s backward pass)."""
+
+    @staticmethod
+    def forward(ctx, x, f0, f1, mode):
+        ctx.taps, ctx.mode, ctx.n = (f0, f1), mode, x.shape[-1]
+        return afb1d_level(x, f0, f1, mode)
+
+    @staticmethod
+    def backward(ctx, dlo, dhi):
+        dx = None
+        if ctx.needs_input_grad[0]:
+            dx = Analysis1DT.apply(dlo, dhi, *ctx.taps, ctx.mode, ctx.n)
+        return dx, None, None, None
+
+
+class Analysis1DT(Function):
+    """``apply(lo, hi, f0, f1, mode, n) -> y``: the transpose of ``Analysis1D`` for a length-n input."""
+
+    @staticmethod
+    def forward(ctx, lo, hi, f0, f1, mode, n):
+        ctx.taps, ctx.mode = (f0, f1), mode
+        return afb1d_adjoint_level(lo, hi, f0, f1, mode, n)
+
+    @staticmethod
+    def backward(ctx, dy):
+        dlo = dhi = None
+        if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
+            dlo, dhi = Analysis1D.apply(dy.contiguous(), *ctx.taps, ctx.mode)
+        return dlo, dhi, None, None, None, None
+
+
 class AFB1D(Function):
     """Single-level 1-D analysis; drop-in for the reference ``AFB1D`` (dwt/lowlevel.py:368-424):
-    ``apply(x, h0, h1, mode) -> (x0, x1)``; backward = synthesis with the same filters, cropped to the input length."""
+    ``apply(x, h0, h1, mode) -> (x0, x1)``; backward = synthesis with the same filters, cropped to the input length
+    (``SynthesisCrop1D``, differentiable to any order)."""
 
     @staticmethod
     def forward(ctx, x, h0, h1, mode):
@@ -72,12 +176,13 @@ class AFB1D(Function):
     def backward(ctx, dx0, dx1):
         dx = None
         if ctx.needs_input_grad[0]:
-            dx = sfb1d_level(dx0, dx1, ctx.taps[0], ctx.taps[1], ctx.mode, out_len=ctx.n)
+            dx = SynthesisCrop1D.apply(dx0, dx1, ctx.taps[0], ctx.taps[1], ctx.mode, ctx.n)
         return dx, None, None, None
 
 
 class SFB1D(Function):
-    """Single-level 1-D synthesis; drop-in for the reference ``SFB1D`` (dwt/lowlevel.py:697-743)."""
+    """Single-level 1-D synthesis; drop-in for the reference ``SFB1D`` (dwt/lowlevel.py:697-743).  Backward = the
+    analysis with the same filters (``Analysis1D``, differentiable to any order)."""
 
     @staticmethod
     def forward(ctx, low, high, g0, g1, mode):
@@ -91,7 +196,7 @@ class SFB1D(Function):
     def backward(ctx, dy):
         dlow = dhigh = None
         if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
-            dlow, dhigh = afb1d_level(dy.contiguous(), ctx.taps[0], ctx.taps[1], ctx.mode)
+            dlow, dhigh = Analysis1D.apply(dy.contiguous(), ctx.taps[0], ctx.taps[1], ctx.mode)
         return dlow, dhigh, None, None, None
 
 
